@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json metric: 256x256x3 slices/sec of the PnP-AdaNet hot path on B200, synthetic data,
+"""bench.py -- BASELINE.json metric: 256x256x3 slices/sec of the PnP-AdaNet hot path on H100, synthetic data,
 random-init weights.
 
     python bench.py --gpus N --steps K --warmup W [--config C]     (N>1: launched by torchrun, one rank per GPU)
@@ -16,6 +16,10 @@ random-init weights.
 Prints ONE JSON line on stdout (rank 0); everything else (per-kernel tables, NCCL's own log when NCCL_DEBUG is set) goes
 to stderr.  `value` = whole-job slices/s with inputs resident in HBM; `e2e` = the same metric through the Trainer API
 with pinned-host inputs copied every step and the loss read back every step.
+
+--dump-outputs DIR writes what the last timed step returned (logits, or the loss terms of the training steps) and a fixed,
+seeded sample of the model variables after it, as DIR/<name>.npy (float32 / float64, < 64 MB in all).  Inputs, weights and
+dropout seeds depend only on the arguments, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -55,9 +59,10 @@ def _peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return {"bf16_tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0)), "hbm_gbs": d.get("hbm_gbs", 6650.0),
+        return {"bf16_tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops", 989.0)), "hbm_gbs": d.get("hbm_gbs", 3350.0),
                 "source": "MEASURED_PEAKS.json (bf16_tflops_sustained: kernel timed inside a long step)"}
-    return {"bf16_tflops": 1590.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s -- a ceiling, not a measured rate
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (dense bf16, 700 W)"}
 
 
 class ClockSampler:
@@ -109,7 +114,7 @@ def bench_config(cfg, B, keep_prob, world, backend=None, graphed=None):
     per_step = {1: B, 2: B, 3: 2 * B, 4: 3 * B, 5: 3 * B}[cfg] * world
     c = {"workload": WORKLOADS[cfg][0], "bench_config": cfg, "batch_per_gpu_per_domain": B, "slices_per_step": per_step,
          "keep_prob": keep_prob if cfg != 1 else 1.0, "parallelism": "dp%d" % world,
-         "l2": "per-step working set (activations of %d slices, GBs) exceeds the 126 MB L2; no explicit flush" % (per_step // world)}
+         "l2": "per-step working set (activations of %d slices, GBs) exceeds the 50 MB L2; no explicit flush" % (per_step // world)}
     return c
 
 
@@ -328,12 +333,14 @@ def run_ours(a):
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = [None]        # what the most recent timed step returned
+
     def timed(fn, steps):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for i in range(steps):
-            fn(i)
+            last[0] = fn(i)
         e1.record()
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1)
@@ -355,6 +362,8 @@ def run_ours(a):
     ms_total = timed(w.step_resident, a.steps)
     launches = launches_per_step * a.steps
     clocks = sampler.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0:
+        _dump_outputs(w, last[0], a.dump_outputs)
     ms_step = ms_total / a.steps
     cfgobj = bench_config(a.config, B, a.keep_prob, world)
     slices_per_step = cfgobj["slices_per_step"]
@@ -391,7 +400,7 @@ def run_ours(a):
             tr.release_graphs()
             w.graphed = False
 
-    # roofline of the dominant kernel (tcgen05 conv): CUDA events around every launch over a few eager steps
+    # roofline of the dominant kernel (tensor-core conv): CUDA events around every launch over a few eager steps
     roof = None
     nprof = min(a.steps, 3)
     if rank == 0:
@@ -431,7 +440,7 @@ def run_ours(a):
         out = {
             "metric": METRIC, "value": value, "unit": "slices/s", "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
             "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": ("bf16 (tcgen05, fp32 accumulate)" if nterms == 1 else "f32 (tcgen05 bf16 hi/lo split x3, fp32 accumulate)"),
+            "dtype": ("bf16 (wgmma, fp32 accumulate)" if nterms == 1 else "f32 (wgmma bf16 hi/lo split x3, fp32 accumulate)"),
             "data": "synthetic", "config": cfgobj,
             "detail": {"conv_backend": a.backend, "cuda_graph": bool(w.graphed or (a.graph and nd20 is not None)),
                        "gflop_per_step_algorithmic": w.gflop_per_step * world},
@@ -461,16 +470,43 @@ def run_ours(a):
         os._exit(0)
 
 
-def _latest_profile(stem):
-    for r in ("r2", "r1"):
-        p = os.path.join(ROOT, "profiles", "%s_%s" % (r, stem))
-        if os.path.exists(p):
-            return p
-    return None
+DUMP_SAMPLE = {"logits": 8 << 20, "variables": 4 << 20}     # elements kept per array: 32 + 16 MB of float32 at most
+
+
+def _sample(t, cap, seed):
+    """t flattened; larger than cap elements -> a fixed, seeded sample of cap of them (sorted indices)"""
+    t = t.detach().reshape(-1)
+    if t.numel() <= cap:
+        return t
+    g = torch.Generator().manual_seed(seed)
+    idx = torch.randperm(t.numel(), generator=g)[:cap].sort().values
+    return t[idx.to(t.device)]
+
+
+def _dump_outputs(w, out, d):
+    """DIR/<name>.npy of what the last timed step computed: the step's return values and the model variables after it"""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    torch.cuda.synchronize()
+    arrays = {}
+    if w.cfg == 1:
+        arrays["logits"] = _sample(out, DUMP_SAMPLE["logits"], 1).float()
+    elif w.cfg == 2:
+        arrays["wce"], arrays["dice"] = out[0].detach().double().reshape(-1), out[1].detach().double().reshape(-1)
+    else:
+        parts = [("dis_loss_terms", out)] if w.cfg == 3 else [("dis_loss_terms", out[0]), ("gen_loss_terms", out[1])]
+        for name, terms in parts:        # [(scalar tensor, weight), ...]; the loss is sum(term * weight)
+            arrays[name] = torch.stack([t.detach().double().reshape(()) * wt for t, wt in terms])
+    if w.cfg != 1:
+        flat = torch.cat([v.detach().float().reshape(-1) for v in w._all_vars()])
+        arrays["variables"] = _sample(flat, DUMP_SAMPLE["variables"], 2)
+    for name, t in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), t.cpu().numpy())
+    print("bench: wrote %s to %s" % (", ".join(sorted(arrays)), d), file=sys.stderr)
 
 
 def _roofline(recs_all, nprof, ms_step, a):
-    recs = [r_ for r_ in recs_all if not r_[3].startswith("simt:")]      # the roofline is the tcgen05 kernel's
+    recs = [r_ for r_ in recs_all if not r_[3].startswith("simt:")]      # the roofline is the tensor-core kernel's
     by_s = {}
     for s_, e_, fl_, tag_, _k in recs_all:
         if tag_.startswith("simt:"):
@@ -498,36 +534,25 @@ def _roofline(recs_all, nprof, ms_step, a):
         c_[2] += fl_
     for k_, (n_, ms_, fl_) in sorted(per_k.items(), key=lambda kv: -kv[1][1]):
         print("[kern] %-34s x%4d %9.3f ms  %7.1f TF/s" % (k_, n_, ms_, fl_ / ms_ / 1e9), file=sys.stderr)
-    print("[conv] tcgen05 %.3f ms/step, simt %.3f ms/step, step %.3f ms" % (all_ms / nprof, simt_ms / nprof, ms_step), file=sys.stderr)
+    print("[conv] tensor-core %.3f ms/step, simt %.3f ms/step, step %.3f ms" % (all_ms / nprof, simt_ms / nprof, ms_step), file=sys.stderr)
     pk = _peaks()
     nterms = 1 if a.backend == "tc1" else 3
     if not recs or all_ms <= 0:
         return {"bound": "tensor", "achieved": 0.0, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": 0.0, "traffic": None,
-                "note": "no tcgen05 launches recorded (backend=%s)" % a.backend}
+                "note": "no tensor-core launches recorded (backend=%s)" % a.backend}
     # the dominant kernel = the instantiation with the largest share of the step (agrees with the committed launch list)
     dom = max(per_k.items(), key=lambda kv: kv[1][1])[0]
     dom_recs = [r_ for r_ in recs if r_[4] == dom]
     tc_ms = sum(r_[0].elapsed_time(r_[1]) for r_ in dom_recs)
     tc_fl = sum(r_[2] for r_ in dom_recs)
-    traffic, traffic_note = None, "no ncu capture committed"
-    tj = _latest_profile("conv_tc_ncu.json")
-    if tj:
-        with open(tj) as f:
-            nj = json.load(f)
-        # captures taken before the CTA-pair variant existed name the single-CTA kernel without its 4th template argument
-        norm = lambda k_: k_.replace(", 1>", ">") if k_.count(",") == 3 else k_
-        mine = [l_ for l_ in nj.get("launches", []) if norm(l_["kernel"]).endswith(norm(dom))]
-        if mine:
-            traffic = sum(l_["dram_bytes"] for l_ in mine) / len(mine)
-            traffic_note = ("dram__bytes_read+write per launch, mean over the %d %s launches of the committed ncu --set full capture "
-                            "(%s; different layers than the event-timed mean, same kernel)" % (len(mine), dom, os.path.relpath(tj, ROOT)))
+    traffic, traffic_note = None, "not measured"
     ach = tc_fl / (tc_ms * 1e-3) / 1e12
     ach_all = all_fl / (all_ms * 1e-3) / 1e12
-    return {"bound": "tensor", "kernel": "%s (tcgen05.mma kind::f16 + TMA, persistent)" % dom, "achieved": ach, "peak": pk["bf16_tflops"],
+    return {"bound": "tensor", "kernel": "%s (wgmma.mma_async bf16 + TMA, persistent)" % dom, "achieved": ach, "peak": pk["bf16_tflops"],
             "unit": "TFLOP/s", "frac": ach / pk["bf16_tflops"], "traffic": traffic, "traffic_note": traffic_note, "peak_source": pk["source"],
             "launches_per_step": len(dom_recs) / nprof, "kernel_ms_per_step": tc_ms / nprof,
             "share_of_step": (tc_ms / nprof) / ms_step, "mma_terms": nterms, "issued_frac": nterms * ach / pk["bf16_tflops"],
-            "all_tcgen05_convs": {"achieved": ach_all, "frac": ach_all / pk["bf16_tflops"], "issued_frac": nterms * ach_all / pk["bf16_tflops"],
+            "all_tensor_core_convs": {"achieved": ach_all, "frac": ach_all / pk["bf16_tflops"], "issued_frac": nterms * ach_all / pk["bf16_tflops"],
                                   "launches_per_step": len(recs) / nprof, "kernel_ms_per_step": all_ms / nprof,
                                   "share_of_step": (all_ms / nprof) / ms_step},
             "note": "achieved = algorithmic 2*M*N*K per launch / event time (eager pass); the fp32-grade path issues mma_terms bf16 "
@@ -639,7 +664,11 @@ def main():
     ap.add_argument("--graph", dest="graph", action="store_true", default=True, help="replay the step as one CUDA graph (default)")
     ap.add_argument("--no-graph", dest="graph", action="store_false")
     ap.add_argument("--profile", action="store_true", help="per-kernel device-time table of two eager steps (torch.profiler) on stderr")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (see the module docstring)")
     a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
     if a.batch is None:
         a.batch = WORKLOADS[a.config][1]
     if a.backend is None:

@@ -1,5 +1,5 @@
 /*
- * pnp_b200.h -- C-ABI of the B200-native (sm_100a) PnP-AdaNet hot path.
+ * pnp_b200.h -- C-ABI of the H100-native (sm_90a) PnP-AdaNet hot path.
  *
  * The reference (carrenD/Medical-Cross-Modality-Domain-Adaptation) is pure Python over TensorFlow-1.4
  * and has no FFI of its own; the narrowest stable seam is the layers.py / ops.py operator surface
@@ -54,14 +54,11 @@ typedef struct {
 
 const char* pnp_error_string(int code);
 int pnp_version(void);
-/* 1 if the loaded library carries the tcgen05/TMA convolution path and the device is sm_100 */
+/* 1 if the loaded library carries the wgmma/TMA convolution path and the device is sm_90 (Hopper) */
 int pnp_tc_available(void);
 /* tile configuration chosen by the most recent pnp_conv2d_tc_fwd / _dgrad call (N tile, K block, split-K factor); lets the
    benchmark attribute each timed launch to a kernel instantiation.  Host-side bookkeeping only. */
 int pnp_tc_last_config(int* block_n, int* block_k, int* ksplit);
-/* 1 if that launch ran as CTA pairs (clusters of 2, tcgen05 cta_group::2: one 256-row MMA per pair of 128-pixel tiles, each CTA
-   staging half of the weight tile); PNP_TC_PAIR selects the tile shapes that may (bit 0: N 256, bit 1: N 128, bit 2: N 64) */
-int pnp_tc_last_pair(void);
 
 /* ---- convolution, general SIMT fp32 path (conv_simt.cu) --------------------------------------
  * replaces tf.nn.conv2d (layers.py:18,24,67,73) and tf.nn.atrous_conv2d (layers.py:86,92) plus
@@ -86,7 +83,7 @@ int pnp_ps_mirror_conv_fwd(const float* X, const float* w, float* y, int B, int 
 int pnp_ps_mirror_conv_bwd(const float* dy, const float* w, float* dX, int B, int a, int b, int G, int r, int kh, int kw,
                            int Cout, int order_b1, void* stream);
 
-/* ---- convolution, tcgen05 + TMA tensor-core path (conv_tc.cu) ----------------------------------
+/* ---- convolution, wgmma + TMA tensor-core path (conv_tc.cu) ------------------------------------
  * Same math as pnp_conv2d_fwd for convolutions whose Cin and Cout are each a multiple of 64, or exactly 32 or 16 (any stride /
  * dilation / kernel <= 5x5; K blocks of 64 / 32 / 16 channels = SWIZZLE_128B / 64B / 32B operand tiles), operands pre-split into
  * bf16 planes (pnp_split_bf16); nterms = 3 gives fp32-grade results (hi*hi + hi*lo + lo*hi), nterms = 1 is the plain bf16 path
@@ -107,7 +104,7 @@ int pnp_conv2d_tc_fwd(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t
 /* Forward convolution with a FUSED epilogue: y = act(dropout(conv) * scale[c] + shift[c] + skip) -- inference-mode batch norm
  * (tf.contrib.layers.batch_norm(is_training=False), layers.py:95-100: scale = gamma*rsqrt(moving_var+eps), shift = beta -
  * moving_mean*scale), the residual add with channel-pad skip (layers.py:160-166) and the activation (layers.py:12-14) applied
- * to the accumulator before it leaves the SM; optionally also emits the bf16 (hi, lo) operand planes of y for the next tcgen05
+ * to the accumulator before it leaves the SM; optionally also emits the bf16 (hi, lo) operand planes of y for the next tensor-core
  * convolution (y itself may then be NULL).  This is the whole frozen-segmenter forward of the D step and the evaluation path
  * (adversarial.py:840-862, 993-1052): one kernel per layer, no z round trip.  ep == NULL: identical to pnp_conv2d_tc_fwd.
  * Batch statistics (bn_sum/bn_sumsq) are statistics of z and cannot be combined with a fused epilogue. */
@@ -124,11 +121,11 @@ int pnp_conv2d_tc_fwd_fused(const uint16_t* x_hi, const uint16_t* x_lo, const ui
                             float* y, const pnp_conv_geom* g, int nterms, const pnp_dropout_cfg* drop, int accumulate,
                             double* bn_sum, double* bn_sumsq, const pnp_tc_epilogue* ep, void* stream);
 
-/* dx[B,H,W,Cin] (+)= conv^T(dy, w) on tcgen05.  g is the FORWARD geometry; stride s > 1 is decomposed into s*s
+/* dx[B,H,W,Cin] (+)= conv^T(dy, w) on the tensor cores.  g is the FORWARD geometry; stride s > 1 is decomposed into s*s
  * stride-1 phase convolutions (no multiplications by the zeros a transposed convolution would insert). */
 int pnp_conv2d_tc_dgrad(const uint16_t* dy_hi, const uint16_t* dy_lo, const uint16_t* w_hi, const uint16_t* w_lo,
                         float* dx, const pnp_conv_geom* g, int nterms, int accumulate, void* stream);
-/* dw[kh][kw][Cin][Cout] += x (*) dy on tcgen05 (both operands MN-major straight from the NHWC planes; pixel range split
+/* dw[kh][kw][Cin][Cout] += x (*) dy on the tensor cores (both operands MN-major straight from the NHWC planes; pixel range split
  * across CTAs, fp32 vector atomics into dw).  x planes are the (mirror-padded) forward input. */
 int pnp_conv2d_tc_wgrad(const uint16_t* x_hi, const uint16_t* x_lo, const uint16_t* dy_hi, const uint16_t* dy_lo,
                         float* dw, const pnp_conv_geom* g, int nterms, int x_channels /* channels of the x planes, 0 = Cin */,
@@ -167,7 +164,7 @@ int pnp_bn_bwd_apply_direct(const float* dy, const float* y, const uint16_t* y_h
                             int training, const pnp_dropout_cfg* drop, float* dgamma, float* dbeta, float* dz, uint16_t* dz_hi,
                             uint16_t* dz_lo, void* stream);
 /* y = act(z*scale + shift + skip);  skip (optional) has Cs channels placed at channel offset skip_off.
- * y_hi / y_lo (optional): also emit the bf16 (hi, lo) operand planes of y for the next tcgen05 convolution */
+ * y_hi / y_lo (optional): also emit the bf16 (hi, lo) operand planes of y for the next tensor-core convolution */
 int pnp_bn_act_apply(const float* z, const float* scale, const float* shift, const float* skip, int Cs,
                      int skip_off, int act, float* y, uint16_t* y_hi, uint16_t* y_lo, long long M, int C, void* stream);
 /* g = dy * act'(y);  sum_g[c] += g;  sum_gx[c] += g * xhat   (xhat = (z-mean)*invstd) */
@@ -177,7 +174,7 @@ int pnp_bn_bwd_reduce(const float* dy, const float* y, const float* z, const flo
 int pnp_bn_bwd_finalize(const double* sum_g, const double* sum_gx, long long M, int C, float* dgamma,
                         float* dbeta, float* coef, void* stream);
 /* training: dz = gamma*invstd*(g - c1 - xhat*c2) ; else dz = gamma*invstd*g ; then * dropout mult.
- * dz_hi / dz_lo (optional): bf16 operand planes of dz for the tcgen05 dgrad / wgrad */
+ * dz_hi / dz_lo (optional): bf16 operand planes of dz for the tensor-core dgrad / wgrad */
 int pnp_bn_bwd_apply(const float* g, const float* z, const float* mean, const float* invstd, const float* gamma,
                      const float* coef, int training, const pnp_dropout_cfg* drop, float* dz, uint16_t* dz_hi, uint16_t* dz_lo,
                      long long M, int C, void* stream);

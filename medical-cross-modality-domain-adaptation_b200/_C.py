@@ -112,7 +112,6 @@ lib.pnp_version.restype = c_int
 lib.pnp_tc_available.restype = c_int
 lib.pnp_tc_last_config.argtypes = [P, P, P]
 lib.pnp_tc_last_config.restype = c_int
-lib.pnp_tc_last_pair.restype = c_int
 
 # launch counter: bench.py reports how many of OUR kernels ran inside the timed region
 launch_count = 0

@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) implementation of the PnP-AdaNet data-parallel hot path
+"""H100-native (sm_90a) implementation of the PnP-AdaNet data-parallel hot path
 (carrenD/Medical-Cross-Modality-Domain-Adaptation): the dilated-residual segmenter forward/backward and
 the feature-map discriminator's adversarial step, behind the reference's layers.py / ops.py operator
 surface and its train_segmenter.py / train_gan.py entry points.

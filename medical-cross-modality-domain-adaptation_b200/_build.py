@@ -1,7 +1,7 @@
-"""In-tree build of the sm_100a shared library (libpnp_b200.so) with nvcc.
+"""In-tree build of the sm_90a (H100) shared library (libpnp_b200.so) with nvcc.
 
-nvcc cross-compiles without a GPU, so this runs in the CPU-only container; the resulting .so is
-git-ignored but travels to the GPU box with the repo snapshot."""
+nvcc cross-compiles without a GPU, so the library can be built on a machine without one; the resulting .so and
+the objects under build/ are git-ignored build products."""
 import os
 import subprocess
 import sys
@@ -12,7 +12,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpnp_b200.so")
 SOURCES = ["conv_simt.cu", "elementwise.cu", "conv_tc.cu", "surface.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(os.path.dirname(HERE), "include", "pnp_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [ "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-diag-suppress", "177"]
 
 
@@ -52,7 +53,7 @@ def build(force=False, verbose=True):
         with ThreadPoolExecutor(max_workers=len(jobs)) as ex:
             list(ex.map(run, jobs))
     if force or jobs or _stale(LIB, objs):
-        run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + objs + ["-cudart", "static"])
+        run([nvcc] + ARCH + ["-shared", "-o", LIB] + objs + ["-cudart", "static"])
     build_io(force, run)
     return LIB
 

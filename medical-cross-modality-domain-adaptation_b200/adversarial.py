@@ -1,4 +1,4 @@
-"""PnP-AdaNet adversarial graph and its alternating D / G training steps -- the B200-native counterpart
+"""PnP-AdaNet adversarial graph and its alternating D / G training steps -- the H100-native counterpart
 of the reference's adversarial.py (Full_DRN :44-574, Trainer :576-1108), eager instead of TF-1 graph.
 
     MR stream : group_1..6 (frozen source segmenter front, BN scopes pred_*)      adversarial.py:130-199

@@ -1,7 +1,10 @@
-// Shared device/host helpers for the PnP-AdaNet B200 hot path (sm_100a only).
+// Shared device/host helpers for the PnP-AdaNet H100 hot path (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+// streaming multiprocessors of an H100 SXM: grid-stride kernels size their grids in multiples of it
+#define PNP_NUM_SMS 132
 
 #define PNP_OK 0
 #define PNP_ERR_BAD_ARG 100001
@@ -28,12 +31,9 @@ static inline int pnp_cdiv(long long a, long long b) { return (int)((a + b - 1) 
 // stream become resident as soon as all CTAs of this one have started (its CTAs take whatever SM resources are free),
 // `griddepcontrol.wait` then blocks until the PREVIOUS kernel has completed and its writes are visible -- no kernel touches
 // global memory before that, so stream-order semantics are kept and only launch latency, CTA scheduling and the per-kernel
-// prologue (the tcgen05 kernels wait after their barrier / TMEM set-up) overlap the predecessor's tail.  With PNP_PDL=1 launches
+// prologue (the tensor-core kernels wait after their barrier set-up) overlap the predecessor's tail.  With PNP_PDL=1 launches
 // carry cudaLaunchAttributeProgrammaticStreamSerialization (stream capture turns it into a programmatic graph edge); without
-// it both instructions are no-ops.  Measured on one B200 (r2t, 20 graph-replayed steps, two repeats): config 4 28.44 ms
-// without vs 28.59 ms with it, config 2 20.22 vs 19.81 ms, config 1 4.39 vs 4.40 ms, config 3 52.17 vs 52.46 ms -- the graph
-// already hides most launch latency and the early-resident dependents cost about what they save: default OFF.  All GPU tests
-// (eager and graph replay) pass in both modes.
+// it both instructions are no-ops.  Inside a CUDA graph most launch latency is already hidden: default OFF.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pnp_pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pnp_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -93,7 +93,7 @@ struct PnpDropout {
 
 // One Philox call yields 128 bits = the 16-bit draws of the EIGHT consecutive elements [8*idx8, 8*idx8+7] (element e uses the
 // low / high half of word (e & 7) >> 1).  16 bits resolve keep_prob to 1.5e-5 (0.75 is exact); halving the Philox calls per
-// element matters in the tcgen05 epilogue, where the mask generation used to cost more issue slots than everything else.
+// element matters in the convolution epilogue, where the mask generation used to cost more issue slots than everything else.
 __device__ __forceinline__ uint4 pnp_dropout_bits8(const PnpDropout& d, unsigned long long seed, unsigned long long idx8) {
   return pnp_philox4x32_10(make_uint4((uint32_t)idx8, (uint32_t)(idx8 >> 32), (uint32_t)d.stream, (uint32_t)(d.stream >> 32)),
                            make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));

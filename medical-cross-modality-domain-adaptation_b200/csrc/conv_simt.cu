@@ -1,9 +1,9 @@
-// General fp32 SIMT implicit-GEMM convolution family for sm_100a.
+// General fp32 SIMT implicit-GEMM convolution family for sm_90a.
 //
 // Replaces tf.nn.conv2d / tf.nn.atrous_conv2d and their gradients as instantiated by the reference's
 // layers.py:18,24,67,73,86,92.  This is the *general* path: any kernel size, stride, dilation,
 // zero-pad offsets and channel counts (Cin = 3, 5, 40 ..., Cout = 5 ...).  The dense stride-1
-// Cin%64==0 layers that carry ~85% of the FLOPs go through the tcgen05 path in conv_tc.cu; the
+// Cin%64==0 layers that carry ~85% of the FLOPs go through the wgmma path in conv_tc.cu; the
 // layers that stay here are the HBM-leaning small-channel ones plus (for now) every wgrad.
 //
 //   fwd   : y[m, n]  = sum_k A(m,k) * Wmat[k, n]         m=(b,oy,ox)  k=(ky,kx,ci)  n=co
@@ -324,7 +324,7 @@ int dispatch_gather(const float* in, const float* wmat, float* out, const Gather
   }
   // grid fill heuristic: prefer the 128x128 tile only when it still yields >= 2 waves
   long long tiles128 = (long long)pnp_cdiv(a.M, 128) * pnp_cdiv(a.OC, 128);
-  if (a.OC <= 64 || tiles128 < 2 * 148) {
+  if (a.OC <= 64 || tiles128 < 2 * PNP_NUM_SMS) {
     if (k16) return launch_gather<128, 64, 16, 8, 4, 4, TR>(in, wmat, out, a, s);
     return launch_gather<128, 64, 8, 8, 4, 4, TR>(in, wmat, out, a, s);
   }
@@ -576,7 +576,7 @@ conv_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dy, flo
 template <int BKK, int BN, int BR, int TK, int TN, int VEC>
 int launch_wgrad(const float* x, const float* dy, float* dw, WgradArgs a, cudaStream_t s) {
   int tiles = pnp_cdiv(a.KK, BKK) * pnp_cdiv(a.Cout, BN);
-  int want = (148 * 6 + tiles - 1) / tiles;             // aim at ~6 CTAs per SM in total
+  int want = (PNP_NUM_SMS * 6 + tiles - 1) / tiles;             // aim at ~6 CTAs per SM in total
   int max_splits = pnp_cdiv(a.M, BR * 4);               // at least 4 reduction blocks per CTA
   int splits = want < 1 ? 1 : want;
   if (splits > max_splits) splits = max_splits;

@@ -1,8 +1,8 @@
-// HBM-bound kernels of the PnP-AdaNet hot path for sm_100a: batch-norm statistics / apply / backward,
+// HBM-bound kernels of the PnP-AdaNet hot path for sm_90a: batch-norm statistics / apply / backward,
 // activation + residual skip, dropout, 2x2 max-pool, mirror pad, phase shift (pixel shuffle) and the
 // discriminator-input gather, per-pixel softmax losses, FC + WGAN means, L2 sums, fused Adam / RMSProp+clip.
 // All are coalesced 128-bit streaming kernels with warp-shuffle / shared-memory reductions and double
-// precision global accumulators; grids are sized in multiples of the 148 SMs.
+// precision global accumulators; grids are sized in multiples of the 132 SMs.
 #include "common.cuh"
 #include "../../include/pnp_b200.h"
 
@@ -10,9 +10,9 @@
 
 namespace {
 
-constexpr int kSMs = 148;
+constexpr int kSMs = PNP_NUM_SMS;
 
-// fp32 -> (hi, lo) bf16 pair with hi + lo ~ x to 2^-17 (operand planes of the tcgen05 convolution, conv_tc.cu)
+// fp32 -> (hi, lo) bf16 pair with hi + lo ~ x to 2^-17 (operand planes of the wgmma convolution, conv_tc.cu)
 __device__ __forceinline__ void split_pair(float x, unsigned short& hi, unsigned short& lo) {
   __nv_bfloat16 h = __float2bfloat16_rn(x);
   __nv_bfloat16 l = __float2bfloat16_rn(x - __bfloat162float(h));
@@ -47,7 +47,7 @@ __device__ __forceinline__ float act_slope(float y, int act) {
 inline int grid_for(long long work_items, int per_block) {
   long long b = (work_items + per_block - 1) / per_block;
   if (b < 1) b = 1;
-  if (b > 148LL * 64) b = 148LL * 64;
+  if (b > PNP_NUM_SMS * 64LL) b = PNP_NUM_SMS * 64LL;
   return (int)b;
 }
 
@@ -1184,7 +1184,7 @@ extern "C" int pnp_bn_bwd_apply_fused(const float* g, const float* z, const floa
 }
 
 /* as pnp_bn_bwd_apply_fused, but from dy: g = dy * act'(y) is recomputed on the fly (activation sign from y or from its bf16 hi
- * plane), so the fp32 g tensor never exists; dz may be NULL when only the bf16 planes are consumed (tcgen05 wgrad / dgrad) */
+ * plane), so the fp32 g tensor never exists; dz may be NULL when only the bf16 planes are consumed (wgmma wgrad / dgrad) */
 extern "C" int pnp_bn_bwd_apply_direct(const float* dy, const float* y, const uint16_t* y_hi, int act, const float* z,
                                        const float* mean, const float* invstd, const float* gamma, const double* sum_g,
                                        const double* sum_gx, long long M, int C, int training, const pnp_dropout_cfg* drop,

@@ -10,7 +10,7 @@ namespace {
 inline int grid_for(long long work_items, int per_block) {
   long long b = (work_items + per_block - 1) / per_block;
   if (b < 1) b = 1;
-  if (b > 148LL * 64) b = 148LL * 64;
+  if (b > PNP_NUM_SMS * 64LL) b = PNP_NUM_SMS * 64LL;
   return (int)b;
 }
 

@@ -1,4 +1,4 @@
-"""Host-side operators of the B200 hot path: thin torch.autograd.Function wrappers whose forward and
+"""Host-side operators of the H100 hot path: thin torch.autograd.Function wrappers whose forward and
 backward are sequences of launches into libpnp_b200.so (include/pnp_b200.h).  PyTorch supplies device
 memory, the stream and the autograd tape; every arithmetic kernel is ours.  NHWC fp32 activations,
 HWIO weights, exactly like the reference (layers.py / ops.py).
@@ -17,11 +17,11 @@ from ._C import call, ptr, ConvGeom, DropCfg
 
 ACT_NONE, ACT_RELU, ACT_LRELU = 0, 1, 2
 
-# fuse BN batch statistics into the tcgen05 conv epilogue (otherwise a separate pnp_bn_stats pass)
+# fuse BN batch statistics into the wgmma conv epilogue (otherwise a separate pnp_bn_stats pass)
 FUSE_BN_STATS = True
 # emit the bf16 operand planes from the BN-apply / BN-backward kernels instead of a separate split pass
 FUSE_SPLIT = os.environ.get("PNP_FUSE_SPLIT", "1") != "0"
-# bench.py sets this to a list to time every tcgen05 launch with CUDA events: (start, end, flops, tag)
+# bench.py sets this to a list to time every wgmma launch with CUDA events: (start, end, flops, tag)
 PROFILE = None
 # debugging aid: callable(sv, dy, g, dz, dx) invoked at the end of every layer_backward
 DEBUG_HOOK = None
@@ -39,7 +39,7 @@ def _tc_launch(tag, flops, name, *args):
     if name in ("pnp_conv2d_tc_fwd", "pnp_conv2d_tc_fwd_fused", "pnp_conv2d_tc_dgrad"):
         n_, k_, s_ = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_int(0)
         _C.lib.pnp_tc_last_config(ctypes.byref(n_), ctypes.byref(k_), ctypes.byref(s_))
-        kern = "conv_tc_kernel<%d, %d, %d, %d>" % (n_.value, 1 if _tc_mode() == 1 else 3, k_.value, 2 if _C.lib.pnp_tc_last_pair() else 1)
+        kern = "conv_tc_kernel<%d, %d, %d>" % (n_.value, 1 if _tc_mode() == 1 else 3, k_.value)
     elif name == "pnp_conv2d_tc_wgrad":
         kern = "conv_wgrad_tc_kernel"
     PROFILE.append((e0, e1, flops, tag, kern))
@@ -91,11 +91,11 @@ def _tc_mode():
     return 1 if b == "tc1" else 3
 
 
-# tcgen05 wgrad can be switched off separately (PNP_TC_WGRAD=0) for A/B measurements
+# wgmma wgrad can be switched off separately (PNP_TC_WGRAD=0) for A/B measurements
 TC_WGRAD = os.environ.get("PNP_TC_WGRAD", "1") != "0"
 TC_PAD32 = os.environ.get("PNP_TC_PAD32", "0") == "1"
-_tc_declined = set()     # (kind, geometry) the tcgen05 launchers returned PNP_ERR_UNSUPPORTED for -> general SIMT kernel
-_tc_proven = set()       # (kind, geometry) that HAVE run on the tcgen05 path: only for those may a producer drop the fp32 copy
+_tc_declined = set()     # (kind, geometry) the wgmma launchers returned PNP_ERR_UNSUPPORTED for -> general SIMT kernel
+_tc_proven = set()       # (kind, geometry) that HAVE run on the tensor-core path: only for those may a producer drop the fp32 copy
 
 
 def _gkey(kind, g):
@@ -110,11 +110,11 @@ def _cin_pad(g):
 
 
 def _tc_ch(c):
-    """channel counts the tcgen05 kernels tile natively: multiples of 64 (128-byte swizzle rows), 32 (64-byte) or 16 (32-byte)"""
+    """channel counts the wgmma kernels tile natively: multiples of 64 (128-byte swizzle rows), 32 (64-byte) or 16 (32-byte)"""
     return c % 64 == 0 or c == 32 or (c == 16 and TC_K16)
 
 
-# the native 32-channel tcgen05 tiles (K block of 32 / N tile of 32); PNP_TC_K32=0 sends those layers back to the SIMT kernel
+# the native 32-channel wgmma tiles (K block of 32 / N tile of 32); PNP_TC_K32=0 sends those layers back to the SIMT kernel
 TC_K32 = os.environ.get("PNP_TC_K32", "1") != "0"
 # 16-channel layers (g1/g2, mask critic): 16-wide K blocks (SWIZZLE_32B).  One TMA instruction moves only 4 KB there, so the
 # kernel is TMA-issue bound and roughly at par with the SIMT kernel (r1p: fwd 256x256 16->16 144 us vs 131 us, dgrad 121 vs 141)
@@ -172,7 +172,7 @@ def _planes_of(x, nterms):
 
 
 def _want_planes(C):
-    """producers emit planes for tensors a tcgen05 convolution is likely to consume (64-multiple channel counts)"""
+    """producers emit planes for tensors a wgmma convolution is likely to consume (64-multiple channel counts)"""
     nt = _tc_mode()
     return nt if (nt and FUSE_SPLIT and (C % 64 == 0 or (C == 32 and TC_K32) or (C == 16 and TC_K32 and TC_K16))) else 0
 
@@ -224,7 +224,7 @@ def _conv_flops(g):
 
 
 class Epilogue:
-    """what the tcgen05 forward convolution may apply to its accumulator before it leaves the SM (pnp_conv2d_tc_fwd_fused):
+    """what the wgmma forward convolution may apply to its accumulator before it leaves the SM (pnp_conv2d_tc_fwd_fused):
     y = act(z * scale + shift + skip), plus the bf16 operand planes of y"""
     __slots__ = ("scale", "shift", "skip", "skip_c", "skip_off", "act", "planes", "planes_only")
 
@@ -236,7 +236,7 @@ class Epilogue:
 
 def conv_fwd_raw(xp, W, geom, drop=None, stats=None, keep_planes=False, ep=None):
     """z = conv(xp, W) [* dropout]; xp already mirror-padded if needed.  stats=(sum,sumsq) f64 buffers are filled only
-    when the tcgen05 path can fuse them.  ep (an Epilogue, tcgen05 path only): the returned tensor is the layer's final y and
+    when the tensor-core path can fuse them.  ep (an Epilogue, tensor-core path only): the returned tensor is the layer's final y and
     carries its planes.  Returns (z or y, stats_done, (hi, lo) bf16 planes of xp or None, epilogue applied)."""
     z = torch.empty(geom.B, geom.Ho, geom.Wo, geom.Cout, dtype=torch.float32, device=xp.device)
     nt = _tc_mode()
@@ -380,14 +380,14 @@ def _geometry(x_shape, w_shape, cfg):
     return p, ConvGeom(B, H, Wd, cin, Ho, Wo, cout, kh, kw, cfg.stride, cfg.dil, pt, pl)
 
 
-# fold inference-mode batch norm + skip + activation into the tcgen05 epilogue (PNP_FUSE_EPILOGUE=0: separate apply kernel)
+# fold inference-mode batch norm + skip + activation into the wgmma epilogue (PNP_FUSE_EPILOGUE=0: separate apply kernel)
 FUSE_EPILOGUE = os.environ.get("PNP_FUSE_EPILOGUE", "1") != "0"
 
 
 def layer_forward(x, W, cfg, skip=None, save=True, planes_only=False):
     """returns (y, saved) -- `saved` is None when save is False (inference / frozen sub-graph).
     planes_only: the caller guarantees that y is consumed ONLY as bf16 operand planes (the hidden activation of a residual
-    block whose second convolution runs on the tcgen05 path): its fp32 copy is then never written, and the backward pass
+    block whose second convolution runs on the tensor-core path): its fp32 copy is then never written, and the backward pass
     takes the activation's sign from the hi plane."""
     x = x.contiguous()
     dev = x.device
@@ -650,7 +650,7 @@ PLANES_ONLY = os.environ.get("PNP_PLANES_ONLY", "1") != "0"
 
 def _hidden_planes_only(x, W1, W2, cfg1, cfg2, save):
     """may the hidden activation h = act(BN(conv1(x))) of a residual block exist as bf16 planes only?  Yes when its single
-    consumer, conv2 (forward, and the weight gradient if W2 trains), has already run on the tcgen05 path for this geometry, h
+    consumer, conv2 (forward, and the weight gradient if W2 trains), has already run on the tensor-core path for this geometry, h
     has a batch norm (whose apply pass / epilogue emits the planes) and the backward pass is the g-less one."""
     if not (PLANES_ONLY and BN_BWD_DIRECT and FUSE_SPLIT and cfg1.bn is not None and cfg2.padding == "SAME" and _tc_mode()):
         return False

@@ -1,5 +1,5 @@
 """Operator surface of the reference's layers.py (same names, argument lists and error behaviour,
-reference file:line cited per function) over torch tensors, executed by the sm_100a kernels in
+reference file:line cited per function) over torch tensors, executed by the sm_90a kernels in
 libpnp_b200.so.  NHWC activations, HWIO weights, strides as 4-lists [1,s,s,1] -- as in the reference.
 
 Differences a TF-1 user must know:

@@ -19,7 +19,7 @@ def init_from_env(backend=None):
         return
     if backend is None:
         backend = "nccl" if torch.cuda.is_available() else "gloo"
-    if torch.cuda.is_available():
+    if backend == "nccl":     # a gloo group (CPU tensors) must not claim a GPU per rank: ranks may outnumber the GPUs
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
     os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
     import datetime

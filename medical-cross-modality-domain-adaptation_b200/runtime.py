@@ -1,4 +1,4 @@
-"""Process-wide runtime state of the B200 hot path: device, stream, dropout RNG, conv backend choice,
+"""Process-wide runtime state of the H100 hot path: device, stream, dropout RNG, conv backend choice,
 and the TF-style variable registry (names follow the reference's checkpoint naming contract,
 lists/half_zip_*_vars, lists/*_bn_list)."""
 import contextlib
@@ -22,8 +22,8 @@ def stream():
 
 
 # ------------------------------------------------------------------------------------------------
-# conv backend: "auto" = tcgen05 (3-term bf16 split) where eligible, SIMT fp32 elsewhere
-#               "simt" = SIMT fp32 everywhere;  "tc1" = tcgen05 single bf16 term (BASELINE config 5)
+# conv backend: "auto" = wgmma (3-term bf16 split) where eligible, SIMT fp32 elsewhere
+#               "simt" = SIMT fp32 everywhere;  "tc1" = wgmma single bf16 term (BASELINE config 5)
 # ------------------------------------------------------------------------------------------------
 _conv_backend = os.environ.get("PNP_CONV_BACKEND", "auto")
 

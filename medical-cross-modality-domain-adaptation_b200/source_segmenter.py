@@ -1,4 +1,4 @@
-"""Source-only dilated-residual segmenter and its Adam training step -- the B200-native counterpart of
+"""Source-only dilated-residual segmenter and its Adam training step -- the H100-native counterpart of
 the reference's source_segmenter.py (Full_DRN :48-301, Trainer :303-675), eager instead of TF-1 graph.
 
 Mapping of the reference's graph attributes (evaluated there through sess.run + feed_dict):

@@ -2,7 +2,7 @@
 for 1 / 4 / 8 / 16 reader threads, CRC check on, files in the page cache (tmpfs when available).  The 8-GPU adversarial step at
 ~800 slices/s/GPU consumes 3 slices of 786 KB per step per GPU-slot: ~5 GB/s for the whole box.
 
-    python scripts/bench_input_pipeline.py [--files 64] [--seconds 3] [--out profiles/r2_input_pipeline.json]
+    python scripts/bench_input_pipeline.py [--files 64] [--seconds 3] [--out result.json]
 """
 import argparse
 import json

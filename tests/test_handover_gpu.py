@@ -4,7 +4,7 @@
       :503-531, :706-765) executed end to end on the GPU and compared with the oracle, whose side of the transplant is done
       independently in numpy from the reference's own name lists (tests/golden/reference_var_names.json = lists/half_zip_*_vars,
       lists/old_bn_list, lists/pred_bn_list);
-  f3  the evaluation path (adversarial.py:894-922 / 993-1052: inference-mode BN -- folded into the tcgen05 epilogue here --,
+  f3  the evaluation path (adversarial.py:894-922 / 993-1052: inference-mode BN -- folded into the wgmma epilogue here --,
       keep_prob 1, hard Dice + confusion matrix) against the oracle.
 """
 import json
@@ -112,7 +112,7 @@ def test_segmenter_checkpoint_hands_over_to_pretrain_discriminator_step(tmp_path
 
 def test_evaluation_path_matches_oracle():
     """Trainer.evaluate: CT slices through the DAM + shared back half in inference mode (every BN folded into its
-    convolution's epilogue on the tcgen05 path), hard Dice with background (lib.py:96-110) and the confusion matrix"""
+    convolution's epilogue on the tensor-core path), hard Dice with background (lib.py:96-110) and the confusion matrix"""
     import pnp_b200  # noqa: F401
     from pnp_b200 import runtime as rt, adversarial as adv, functional as F
     from pnp_b200.train_gan import configure

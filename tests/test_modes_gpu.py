@@ -1,5 +1,5 @@
 """Opt-in launch modes of the C-ABI library, each in its own process (the switches are read once per process):
-PNP_PDL=1 (programmatic dependent launch on every kernel), PNP_TC_PAIR=7 (CTA pairs on the 128x256, 128x128 and 128x64 tiles) and
+PNP_PDL=1 (programmatic dependent launch on every kernel) and
 PNP_TAIL5=3 / 0 (register-tiled 5x5 tail kernels in both directions -- the default, set explicitly here -- / the generic tail kernels) must give the same operator parity as the defaults, eagerly and through CUDA-graph replay."""
 import os
 import subprocess
@@ -22,9 +22,9 @@ def _run(env_extra, args):
 
 
 @pytest.mark.timeout(900)
-def test_operator_parity_with_pdl_and_all_pair_shapes():
-    tail = _run({"PNP_PDL": "1", "PNP_TC_PAIR": "7", "PNP_TAIL5": "3"},
-                ["tests/test_ops_gpu.py", "-k", "tensor_core or cta_pair or fused_epilogue or residual or conv_bn or tail"])
+def test_operator_parity_with_pdl():
+    tail = _run({"PNP_PDL": "1", "PNP_TAIL5": "3"},
+                ["tests/test_ops_gpu.py", "-k", "tensor_core or wide_layers or fused_epilogue or residual or conv_bn or tail"])
     print(tail)
 
 

@@ -97,7 +97,7 @@ TC_CASES = [
     (5, 16, 16, 512, 512, 3, 1, 1, "SAME"),     # cls_5: 16x16 images, 8 rows per tile
     (9, 4, 4, 128, 64, 3, 1, 1, "SAME"),        # tiny images: 8 images per tile, ragged batch
     (2, 64, 64, 32, 64, 3, 1, 1, "SAME"),       # Cin = 32 (cls_1 res a): zero-padded 64-channel planes, fwd + wgrad
-    (8, 32, 32, 256, 512, 3, 1, 1, "SAME"),     # enough tiles for the 128x256 accumulator variant (fwd); dgrad N = 256 too
+    (8, 32, 32, 256, 512, 3, 1, 1, "SAME"),     # 128x128 tiles over 4 n-tiles (fwd), 2 n-tiles (dgrad)
     # strided layers: forward through TMA element strides, dgrad as s*s phase convolutions, wgrad with strided x boxes
     (2, 32, 32, 64, 64, 3, 2, 1, "SAME"),       # cls_x_3 style 3x3 s2, pad (0,1)
     (2, 32, 32, 128, 128, 5, 2, 1, "SAME"),     # cls_2_3: 5x5 s2, pad (1,2)
@@ -116,21 +116,21 @@ TC_CASES = [
     (2, 32, 32, 16, 32, 3, 1, 1, "SAME"),       # g2 inc: forward N 32 / K 16, dgrad N 16 / K 32
     (1, 256, 256, 16, 16, 3, 1, 1, "SAME"),     # g1 at full width
     (8, 32, 32, 16, 32, 5, 4, 1, "SAME"),       # m_cls_2_3: 5x5 stride 4, phase dgrad with N = 16
-    # CTA pairs (cta_group::2): more tile pairs than the 74 clusters of a B200, so every pair walks several tiles
-    (16, 32, 32, 512, 512, 3, 1, 2, "SAME"),    # g8 at config 1's batch: 128 m-tiles x 2 n-tiles of 128x256, dilated
-    (4, 64, 64, 128, 128, 3, 1, 1, "SAME"),     # 128x128 tiles (PNP_TC_PAIR bit 1)
-    (2, 128, 128, 64, 64, 3, 1, 1, "SAME"),     # 128x64 tiles (PNP_TC_PAIR bit 2)
+    # more tiles than the 132 SMs of an H100, so every persistent CTA walks several tiles (and changes n-tile on the way)
+    (16, 32, 32, 512, 512, 3, 1, 2, "SAME"),    # g8 at config 1's batch: 128 m-tiles x 4 n-tiles of 128x128, dilated
+    (4, 64, 64, 128, 128, 3, 1, 1, "SAME"),     # 128x128 tiles
+    (2, 128, 128, 64, 64, 3, 1, 1, "SAME"),     # 128x64 tiles
 ]
 
 
 @pytest.mark.parametrize("case", TC_CASES, ids=lambda c: "B%d_%dx%d_%d-%d_k%d_s%d_d%d_%s" % c)
 @pytest.mark.parametrize("backend,tol", [("tc3", 2e-4), ("tc1", 3e-2)])
 def test_conv_tensor_core(case, backend, tol):
-    """tcgen05 path (3-term split = fp32-grade, 1-term = plain bf16) forward + dgrad vs oracle"""
+    """tensor-core path (3-term split = fp32-grade, 1-term = plain bf16) forward + dgrad vs oracle"""
     L, ops, F, rt = _prod()
     T = _oracle()
     if not rt.tc_available():
-        pytest.fail("tcgen05 path unavailable on this device -- it must be the one that runs on B200")
+        pytest.fail("wgmma path unavailable on this device -- it must be the one that runs on H100")
     rt.set_conv_backend(backend)
     B, H, W, Cin, Cout, k, s, d, pad = case
     F.TC_PAD32 = True          # exercise the zero-padded 64-channel plane path for the Cin = 32 case
@@ -147,17 +147,15 @@ def test_conv_tensor_core(case, backend, tol):
     check("dx", xg.grad, xo.grad, tol)
     check("dw", wg.grad, wo.grad, tol)
     F.TC_PAD32 = False
-    assert not F._tc_declined, "these shapes must run on tcgen05: %s" % (F._tc_declined,)
+    assert not F._tc_declined, "these shapes must run on the tensor cores: %s" % (F._tc_declined,)
     rt.set_conv_backend("auto")
 
 
-def test_cta_pair_kernel_is_selected_for_the_wide_layers():
-    """the 512-channel 32x32 layers of the segmenter (the step's dominant launches) run as CTA pairs unless PNP_TC_PAIR=0"""
-    import os
+def test_wide_layers_select_the_128_column_tile():
+    """the 512-channel 32x32 layers of the segmenter (the step's dominant launches) run on the widest tile, 128x128 with
+    64-channel K blocks, without split-K"""
     L, ops, F, rt = _prod()
     from pnp_b200 import _C
-    if not (int(os.environ.get("PNP_TC_PAIR", "1")) & 1):
-        pytest.skip("PNP_TC_PAIR disables the 128x256 pair kernel")
     rt.set_conv_backend("tc3")
     x, w = randn((8, 32, 32, 512), 3).to(DEV), randn((3, 3, 512, 512), 4, 0.05).to(DEV)
     with torch.no_grad():
@@ -165,7 +163,7 @@ def test_cta_pair_kernel_is_selected_for_the_wide_layers():
     torch.cuda.synchronize()
     n_, k_, s_ = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_int(0)
     _C.lib.pnp_tc_last_config(ctypes.byref(n_), ctypes.byref(k_), ctypes.byref(s_))
-    assert (n_.value, k_.value, s_.value) == (256, 32, 1) and _C.lib.pnp_tc_last_pair() == 1
+    assert (n_.value, k_.value, s_.value) == (128, 64, 1)
     ref = torch.nn.functional.conv2d(x.permute(0, 3, 1, 2).double(), w.permute(3, 2, 0, 1).double(), padding=1).permute(0, 2, 3, 1)
     assert float((y.double() - ref).abs().max() / ref.abs().max()) < 2e-5
     rt.set_conv_backend("auto")
@@ -202,7 +200,7 @@ def test_conv_bn_relu(is_train, leak, backend):
     bn = _bn_pair(T, Cout, 23)
     xo, wo = x.double().requires_grad_(True), w.double().requires_grad_(True)
     mm0, mv0 = bn.moving_mean.clone(), bn.moving_var.clone()
-    st = 1 if backend == "auto" else 2          # stride 1 rides the tcgen05 path (+ fused BN statistics)
+    st = 1 if backend == "auto" else 2          # stride 1 rides the tensor-core path (+ fused BN statistics)
     yo = T.conv_bn_relu2d(xo, wo, 1.0, bn, strides=(1, st, st, 1), is_train=is_train, leak=leak)
     r = randn(tuple(yo.shape), 24)
     (yo * r.double()).sum().backward()
@@ -274,12 +272,12 @@ def test_residual_blocks(inc_dim, kind, is_train, backend):
 
 
 def test_fused_bn_stats_match_separate_pass():
-    """BN statistics reduced in the tcgen05 epilogue == the standalone pnp_bn_stats pass"""
+    """BN statistics reduced in the wgmma epilogue == the standalone pnp_bn_stats pass"""
     L, ops, F, rt = _prod()
     rt.reset_default_graph()
     rt.set_conv_backend("tc3")
     _fused_vs_separate(L, F, rt, randn((3, 32, 32, 64), 41), randn((3, 3, 64, 128), 42, 0.1))
-    # enough tiles for the 128x256 accumulator variant of the persistent kernel (two TMEM buffers of 256 columns)
+    # enough tiles that every persistent CTA walks several 128x128 tiles and changes n-tile on the way
     _fused_vs_separate(L, F, rt, randn((8, 32, 32, 256), 43), randn((3, 3, 256, 512), 44, 0.05))
     rt.set_conv_backend("auto")
 
@@ -589,13 +587,13 @@ def test_dropout_statistics_and_backward_consistency():
     rt.set_conv_backend("auto")
 
 
-# (B, H, W, Cin, Cout, stride, dil, inc_dim skip) -- one case per accumulator tile width of the tcgen05 kernel
+# (B, H, W, Cin, Cout, stride, dil, inc_dim skip) -- one case per accumulator tile width of the wgmma kernel
 FUSED_EP_CASES = [
     (8, 32, 32, 256, 512, 1, 1, True),     # N = 256 tile (8 epilogue warps x 4 chunks), channel-pad skip
     (3, 32, 32, 64, 128, 1, 2, True),      # N = 128, dilated
     (2, 64, 64, 64, 64, 1, 1, False),      # N = 64, same-width skip
     (2, 64, 64, 32, 32, 1, 1, False),      # N = 32 (4 epilogue warps)
-    (2, 64, 64, 16, 16, 1, 1, False),      # N = 16 (16-column tcgen05.ld)
+    (2, 64, 64, 16, 16, 1, 1, False),      # N = 16 (m64n16 wgmma)
     (4, 32, 32, 64, 64, 2, 1, None),       # strided, no skip
 ]
 
@@ -603,7 +601,7 @@ FUSED_EP_CASES = [
 @pytest.mark.parametrize("case", FUSED_EP_CASES)
 @pytest.mark.parametrize("keep_prob", [1.0, 0.75])
 def test_fused_epilogue_equals_separate_bn_apply(case, keep_prob):
-    """inference-mode BN + skip + leaky relu folded into the tcgen05 epilogue (pnp_conv2d_tc_fwd_fused) == convolution followed by
+    """inference-mode BN + skip + leaky relu folded into the wgmma epilogue (pnp_conv2d_tc_fwd_fused) == convolution followed by
     the streaming pnp_bn_apply_fused pass: same fp32 operations in the same order (y to 1e-6, its bf16 planes must re-compose y to
     2^-16); the backward pass (which no longer has z) must give the same gradients."""
     L, ops, F, rt = _prod()

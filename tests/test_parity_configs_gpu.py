@@ -2,7 +2,7 @@
 seeded synthetic inputs and identical initial variables:
 
   config 4, B = 8/GPU, backend auto, through Trainer.capture_joint_step REPLAY -- the first model-level exercise of the
-            dominant 128x256 tcgen05 tile (needs >= 96 tiles, i.e. B >= 6) and of the CUDA-graph path on the tcgen05 backend
+            dominant 128x128 wgmma tile at the benchmarked batch and of the CUDA-graph path on the wgmma backend
   config 2, B = 16: segmenter Adam steps (losses, logits)
   config 3, B = 32 per domain: pre-train D step (dis_loss, updated critic variables)
   config 5: the plain-bf16 (one MMA term) path -- its model-level deviation from the fp32 reference, stated and bounded
@@ -97,13 +97,13 @@ def test_config4_b8_tcgen05_graph_replay_matches_oracle():
     B = 8
     net, trainer, oracle = adv_pair("auto", 0.3, "train-gan", B)
     mr, ct, ct2 = synthetic_images(B, 1234), synthetic_images(B, 4321, 0.3, 0.8), synthetic_images(B, 8765, 0.3, 0.8)
-    # the 128x256 tile must actually be selected at this batch (it is the benchmark's dominant kernel)
+    # the 128x128 tile must actually be selected at this batch (it is the benchmark's dominant kernel)
     F.PROFILE = []
     assert trainer.capture_joint_step(mr.to(DEV), ct.to(DEV), keep_prob=1.0, warmup=1), "CUDA-graph capture failed"
     kerns = {r[4] for r in F.PROFILE}
     F.PROFILE = None
     print("  conv kernels in the step:", sorted(kerns))
-    assert any(k.startswith("conv_tc_kernel<256") for k in kerns), kerns
+    assert any(k.startswith("conv_tc_kernel<128") for k in kerns), kerns
     ro_d, ro_g = oracle.d_step(mr, ct, 1.0), oracle.g_step(ct, 1.0)          # the warm-up step (G on the D step's CT batch)
     for k in range(2):
         d, g = trainer.joint_step(mr.to(DEV), ct.to(DEV), keep_prob=1.0, ct_batch_g=ct2.to(DEV))

@@ -1,11 +1,11 @@
-"""Multi-step parity: do the tcgen05 path's (4-5x noisier than fp32) gradients make a training run drift?
+"""Multi-step parity: do the tensor-core path's (4-5x noisier than fp32) gradients make a training run drift?
 
   * adversarial, 10 free-running joint steps (RMSProp): dis_loss / gen_loss of every step within 1e-3 (of scale) of the fp32
     oracle, variables within 1e-3 at the end.  The fp32 oracle itself drifts from an fp64 one by 1e-5 .. 1.4e-3 of scale over
     these 10 steps (scripts/oracle_trajectory_calibration.py -> tests/golden/oracle_trajectory_calibration.json: it crosses
     1e-3 at steps 6-8); the bf16-split tensor-core path carries ~1e-5 per convolution where fp32 carries ~1e-7, and the WGAN
     loss is a difference of critic means (a single evaluation already sits 1e-4 .. 4e-4 of scale from the oracle on BOTH the
-    fp32 SIMT and the tcgen05 path, tests/test_models_gpu.py).  Per-step bound: max(3e-3, 10 x that step's fp32-vs-fp64 drift)
+    fp32 SIMT and the tensor-core path, tests/test_models_gpu.py).  Per-step bound: max(3e-3, 10 x that step's fp32-vs-fp64 drift)
     -- the same factor 10 the first-step gradient checks grant this path; what the test must show is that the deviation STAYS
     at the 1e-3 level over 10 updates instead of compounding.
   * segmenter, 10 Adam steps.  Adam's update is lr*m/sqrt(v) ~ lr*sign(g): elements whose gradient sits at the fp32 noise floor
@@ -20,7 +20,7 @@
   * held-out Dice gate (north_star): train the segmenter on label-correlated synthetic slices on the GPU, hand the trained
     variables to the oracle, evaluate both on 64 held-out slices (seed 7777): hard Dice (lib.py:96-110) within 1e-3 per
     class, per batch and in the mean.  The checkpoint evaluated is the first one on which hard Dice is insensitive to fp32
-    rounding (measured oracle-free, between the product's tcgen05 and SIMT convolution paths): a model with thousands of
+    rounding (measured oracle-free, between the product's wgmma and SIMT convolution paths): a model with thousands of
     pixels within rounding of a tie separates no two fp32 implementations to 1e-3 (see the comment in the test).
 """
 import json
@@ -155,8 +155,8 @@ def test_held_out_dice_gate_seed_7777():
 
     def rounding_sensitivity():
         """How far does fp32-level rounding move the hard Dice of THIS model?  Measured without the oracle: the same forward on
-        the two independent convolution implementations of the product (tcgen05 bf16-split tiles vs the fp32 SIMT direct
-        convolution; they differ from each other by what the tcgen05 path differs from the oracle, tests/test_ops_gpu.py).
+        the two independent convolution implementations of the product (wgmma bf16-split tiles vs the fp32 SIMT direct
+        convolution; they differ from each other by what the tensor-core path differs from the oracle, tests/test_ops_gpu.py).
         -> (worst |dDice| over batches and classes between the two, re-labelled pixels, mean held-out Dice)"""
         worst, flips, dices = 0.0, 0, []
         with torch.no_grad():
@@ -194,7 +194,7 @@ def test_held_out_dice_gate_seed_7777():
         # one.  So: evaluate the first checkpoint whose Dice does not move by more than a quarter of the gate between the
         # product's own two convolution implementations (else the least sensitive one of 12).
         sens, flips, dv = rounding_sensitivity()
-        print("  after %3d Adam steps on the GPU: wce %.4f dice-loss %.4f ; held-out Dice %.4f ; tcgen05 vs SIMT forward: %d re-labelled pixels, worst |dDice| %.2e"
+        print("  after %3d Adam steps on the GPU: wce %.4f dice-loss %.4f ; held-out Dice %.4f ; wgmma vs SIMT forward: %d re-labelled pixels, worst |dDice| %.2e"
               % (steps, float(wce), float(dice), dv, flips, sens))
         if dv > 0.5 and (best is None or sens < best[0]):
             best = (sens, steps, rt.state_dict())

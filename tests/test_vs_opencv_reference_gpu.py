@@ -5,7 +5,7 @@ stream of `adversarial.Full_DRN` (create_zip_network + create_second_half), comp
 GraphDef that was built out of the recorded trace of the reference's own graph-building code
 (tests/golden/make_opencv_reference_vectors.py; tests/test_reference_graph_in_opencv_cpu.py checks the same numbers against the oracle
 on the CPU).  Here the product runs the same seeded parameters and inputs on the GPU -- inference-mode batch norm folded into the
-tcgen05 epilogues, fused tail -- and must reproduce them: logits within 1e-3 of the largest |logit| (north-star tolerance), argmax maps
+wgmma epilogues, fused tail -- and must reproduce them: logits within 1e-3 of the largest |logit| (north-star tolerance), argmax maps
 equal on >= 99.9 % of the pixels."""
 import numpy as np
 import pytest
