@@ -89,7 +89,9 @@ int pnp_ps_mirror_conv_bwd(const float* dy, const float* w, float* dX, int B, in
  * bf16 planes (pnp_split_bf16); nterms = 3 gives fp32-grade results (hi*hi + hi*lo + lo*hi), nterms = 1 is the plain bf16 path
  * of BASELINE config 5.  Unsupported shapes return PNP_ERR_UNSUPPORTED (the caller then uses pnp_conv2d_*).  Layers with very
  * few tiles and a deep reduction are split along K inside the call (atomic accumulation into a zeroed y; bn_sum/bn_sumsq are then
- * produced by an internal pnp_bn_stats pass).  The weight gradient takes Cin in {32, 64k} and Cout = 64k. */
+ * produced by an internal pnp_bn_stats pass).  bn_sum/bn_sumsq with accumulate != 0 returns PNP_ERR_BAD_ARG: the statistics
+ * would be of the new contribution on one path and of old + new on the other.  The weight gradient takes Cin in {32, 64k} and
+ * Cout = 64k. */
 int pnp_split_bf16(const float* x, uint16_t* hi, uint16_t* lo, long long n, void* stream);
 /* w HWIO fp32 -> bf16 planes: for_dgrad == 0: [tap][Cout][Cin] (K-major B operand of the forward conv);
  * for_dgrad != 0: [tap][Cin][Cout] (K-major B operand of the data gradient) */

@@ -1105,6 +1105,8 @@ extern "C" int pnp_conv2d_tc_fwd_fused(const uint16_t* x_hi, const uint16_t* x_l
   if (nterms != 1 && nterms != 3) return PNP_ERR_BAD_ARG;
   if (nterms == 3 && (!x_lo || !w_lo)) return PNP_ERR_BAD_ARG;
   if ((bn_sum == nullptr) != (bn_sumsq == nullptr)) return PNP_ERR_BAD_ARG;
+  // the epilogue reduces the statistics of the new contribution, the split-K path those of old + new: no single meaning
+  if (accumulate && bn_sum) return PNP_ERR_BAD_ARG;
   if (!tc_geom_ok(g)) return PNP_ERR_UNSUPPORTED;
   TcArgs a;
   a.B = g->B; a.OH = g->Ho; a.OW = g->Wo; a.Cout = g->Cout; a.Cin = g->Cin;
