@@ -305,6 +305,9 @@ struct TcCfg {
   static_assert(SMEM_BYTES <= 227 * 1024, "H100 allows 227 KB of shared memory per block");
 };
 
+// 32-bit word k (0..3, may differ per lane) of a Philox block
+__device__ __forceinline__ uint32_t word_of(const uint4& r, int k) { return k == 0 ? r.x : k == 1 ? r.y : k == 2 ? r.z : r.w; }
+
 template <int BLOCK_N, int NTERMS, int BK>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
@@ -380,17 +383,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   // wgmma accumulator layout (m64nN, fp32): thread (warp w of the warpgroup, lane l) holds rows 16w + l/4 and 16w + l/4 + 8,
   // and of every 8-column group j the columns 8j + 2(l%4) + {0, 1}: d[4j + {0,1}] in the first row, d[4j + {2,3}] in the second
   const int wg = warp >> 2;
-  const int cq = (lane & 3) * 2;
+  const int q = lane & 3;
+  const int cq = q * 2;
   const int per_img = a.th * a.tw;
-  int rni[2], ryy[2], rxx[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int m = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;     // accumulator row = pixel index inside the tile
-    rni[h] = m / per_img;
-    const int rem = m - rni[h] * per_img;
-    ryy[h] = rem / a.tw;
-    rxx[h] = rem - ryy[h] * a.tw;
-  }
   const bool drop_on = a.drop.seed_ptr != nullptr;
   unsigned long long seed = 0ull;
   if (drop_on) seed = *a.drop.seed_ptr;
@@ -463,14 +458,47 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
       if (lane == 0) mbar_arrive(smem_u32(&bars[STAGES + prev]));
     }
 
+    // the rows' coordinates are derived per tile rather than kept live across the K loop
     long long pix[2];
     bool valid[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int img = tc.img0 + rni[h], u = tc.y0 + ryy[h], v_ = tc.x0 + rxx[h];
-      valid[h] = (rni[h] < a.tn) && (img < a.B) && (u < tc.U) && (v_ < tc.V);
+      const int m = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;     // accumulator row = pixel index inside the tile
+      const int rni = m / per_img;
+      const int rem = m - rni * per_img;
+      const int ryy = rem / a.tw;
+      const int img = tc.img0 + rni, u = tc.y0 + ryy, v_ = tc.x0 + (rem - ryy * a.tw);
+      valid[h] = (rni < a.tn) && (img < a.B) && (u < tc.U) && (v_ < tc.V);
       const int oy = u * a.out_mul + tc.py, ox = v_ * a.out_mul + tc.px;
       pix[h] = ((long long)img * a.OH + oy) * a.OW + ox;
+    }
+    if (drop_on) {
+      // element e draws half (e & 1) of word (e & 7) >> 1 of the Philox block e >> 3 (pnp_dropout_mult8), so the four lanes of
+      // a quad (one row; columns 2q, 2q + 1 of every 8-column group) need the same block, word q each.  Lane q draws the block
+      // of group 4 jg + q, and three xor shuffles transpose the quad's 4 x 4 words: got[s] = word q of the block of group
+      // 4 jg + (q ^ s).  Invalid rows (and, at 16 columns, the groups past the tile) draw too, unused, so that every lane
+      // reaches every shuffle.
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const unsigned long long blk0 = (unsigned long long)(pix[h] * a.Cout + n0 + q * 8) >> 3;
+#pragma unroll
+        for (int jg = 0; jg < (BLOCK_N / 8 + 3) / 4; ++jg) {
+          const uint4 blk = pnp_dropout_bits8(a.drop, seed, blk0 + 4 * jg);
+          uint32_t got[4];
+          got[0] = word_of(blk, q);
+#pragma unroll
+          for (int s = 1; s < 4; ++s) got[s] = __shfl_xor_sync(0xffffffffu, word_of(blk, q ^ s), s);
+#pragma unroll
+          for (int jq = 0; jq < 4; ++jq) {
+            const int j = 4 * jg + jq;
+            if (j >= BLOCK_N / 8) break;
+            const int sj = q ^ jq;
+            const uint32_t w = sj == 0 ? got[0] : sj == 1 ? got[1] : sj == 2 ? got[2] : got[3];
+            acc[4 * j + 2 * h] *= pnp_drop_sel(a.drop, w & 0xffffu);
+            acc[4 * j + 2 * h + 1] *= pnp_drop_sel(a.drop, w >> 16);
+          }
+        }
+      }
     }
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; ++j) {
@@ -481,17 +509,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
       for (int h = 0; h < 2; ++h) {
         v[h][0] = acc[4 * j + 2 * h];
         v[h][1] = acc[4 * j + 2 * h + 1];
-      }
-      if (drop_on) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (!valid[h]) continue;
-          // the draw of element e is half (e & 1) of word (e & 7) >> 1 of the Philox block e >> 3 (pnp_dropout_mult8)
-          const uint4 r = pnp_dropout_bits8(a.drop, seed, (unsigned long long)(pix[h] * a.Cout + n0 + j * 8) >> 3);
-          const uint32_t w = (cq == 0) ? r.x : (cq == 2) ? r.y : (cq == 4) ? r.z : r.w;
-          v[h][0] *= pnp_drop_sel(a.drop, w & 0xffffu);
-          v[h][1] *= pnp_drop_sel(a.drop, w >> 16);
-        }
       }
       if (bn_on) {
         float s0 = (valid[0] ? v[0][0] : 0.f) + (valid[1] ? v[1][0] : 0.f);
