@@ -229,6 +229,18 @@ int pnp_logits_argmax_concat(const float* logits, float* out, long long P, int C
 /* ---- losses and metrics ---------------------------------------------------------------------------- */
 /* layers.py:134-138 */
 int pnp_pixel_softmax2(const float* logits, float* out, long long P, int C, void* stream);
+/* tf.summary.image(name, tf.expand_dims(tf.cast(t, tf.float32), 3)) panels of one monitoring pass in one launch
+ * (source_segmenter.py:398-405, adversarial.py:676-687; TF-1.4 ImageSummaryOp, float path, normalised per image).  Source s is
+ * srcs[s] = fp32 NHWC [B, H, W, C[s]] and kinds[s] says which single-channel image it shows:
+ *   PNP_IMG_CHANNEL          channel channel[s] (the x[:,:,:,1] input slice);
+ *   PNP_IMG_ARGMAX           float(first-max index over the C[s] <= 8 channels) (tf.argmax of a one-hot label map);
+ *   PNP_IMG_SOFTMAX2_ARGMAX  float(first-max index over pnp_pixel_softmax2 of the C[s] <= 8 logits) (compact_pred).
+ * Images 0..n-1 (n = min(B, max_outputs) <= B) of up to 6 sources go to out[nsrc][n][H*W] (uint8). */
+#define PNP_IMG_CHANNEL 0
+#define PNP_IMG_ARGMAX 1
+#define PNP_IMG_SOFTMAX2_ARGMAX 2
+int pnp_image_summary_u8(const float* const* srcs, const int* kinds, const int* C, const int* channel, int nsrc,
+                         int B, int H, int W, int n, unsigned char* out, void* stream);
 /* source_segmenter.py:241-273: per-class partial sums acc[4*C] (doubles, zeroed by caller):
  * [0,C) sum y ; [C,2C) sum p*y ; [2C,3C) sum p*p ; [3C,4C) sum -y*log(clip(p,.005,1)) */
 int pnp_segloss_reduce(const float* logits, const float* y, long long P, int C, double* acc, void* stream);

@@ -86,6 +86,7 @@ SIGNATURES = {
     "pnp_logits_argmax_concat": [P, P, c_ll, c_int, c_int, c_int, P],
     "pnp_disc_input_fwd": [P, P, P, P, P, c_int, P, c_int, P, c_int, c_int, c_int, c_int, c_int, P],
     "pnp_pixel_softmax2": [P, P, c_ll, c_int, P],
+    "pnp_image_summary_u8": [P, P, P, P, c_int, c_int, c_int, c_int, c_int, P, P],
     "pnp_segloss_reduce": [P, P, c_ll, c_int, P, P],
     "pnp_segloss_finalize": [P, c_ll, c_int, P, P, P],
     "pnp_segloss_bwd": [P, P, P, P, P, P, c_ll, c_int, P],

@@ -450,12 +450,21 @@ class Trainer(object):
     # the reference's TensorBoard scalar tags (adversarial.py:664-683), written as JSON lines because TensorBoard is not a dependency
     SCALAR_TAGS = ("fixed_coeff_reg", "discriminator_loss", "generator_loss", "ct_dice_eval_c1_lv_myo", "ct_dice_eval_c2_la_blood",
                    "ct_dice_eval_c3_lv_blood", "ct_dice_eval_c4_aa", "mri_dice", "learning_rate")
+    # image summaries of train_image_summary_op, in its order (adversarial.py:676-682): [compact_pred, ct[:,:,:,1], compact_y,
+    # compact_mr_valid, mr[:,:,:,1], compact_mr_y].  output_minibatch_stats fetches this op on every pass, the validation pass
+    # (detail=True) included; val_image_summary_op (adversarial.py:684-687, its 'ct_image' uniquified to 'ct_image_1') is built
+    # but never fetched, so VAL_IMAGE_TAGS is never written
+    TRAIN_IMAGE_TAGS = ("ct_pred", "ct_image", "ct_gt", "mri_validation_pred", "mri_image", "mri_gt")
+    VAL_IMAGE_TAGS = ("ct_val_pred", "ct_image_1", "ct_val_gt")
 
-    def output_minibatch_stats(self, step, ct_batch, ct_batch_y, mr_batch, mr_batch_y, log_dir=None, detail=False):
+    def output_minibatch_stats(self, step, ct_batch, ct_batch_y, mr_batch, mr_batch_y, log_dir=None, detail=False,
+                               image_summaries=False):
         """adversarial.py:948-990, scalar part: one monitoring pass with the segmenter in inference mode and keep_prob 1 (the feed
         also sets cls_bn False, but create_classifier / create_mask_critic never read that placeholder: the critics run with
         their hard-wired batch-statistics BN -- moving averages move -- and keep_prob 0.75, reproduced).  Returns the scalars under
-        the reference's tags and appends them to <log_dir>/scalars.jsonl; detail=True also prints per-organ Dice / Jaccard."""
+        the reference's tags and appends them to <log_dir>/scalars.jsonl; detail=True also prints per-organ Dice / Jaccard.
+        `image_summaries` writes the TRAIN_IMAGE_TAGS panels of this pass's own forwards to the event file after the scalars,
+        with the same step (add_summary(summary_str, step); add_summary(summary_img, step))."""
         import json
         from .lib import _indicator_eval
         net = self.net
@@ -483,13 +492,18 @@ class Trainer(object):
         if detail:
             _indicator_eval(cm.cpu().numpy())
         if log_dir is not None and self.dp.rank == 0:
-            # summary_writer.add_summary(summary_str, step); flush() (adversarial.py:989-991): a TensorBoard event file (scalars only)
-            # and the same numbers as one JSON line
-            from .summary import FileWriter
+            # summary_writer.add_summary(summary_str, step); add_summary(summary_img, step); flush() (adversarial.py:989-991): a
+            # TensorBoard event file and the same scalars as one JSON line
+            from .summary import FileWriter, image_tags
             writers = self.__dict__.setdefault("_summary_writers", {})
             if log_dir not in writers:
                 writers[log_dir] = FileWriter(log_dir)
             writers[log_dir].add_scalars(scalars, step)
+            if image_summaries:
+                u8 = F.image_summary([(fc_["logits"], "softmax2_argmax", 0), (ct_batch, "channel", 1), (ct_batch_y, "argmax", 0),
+                                      (fm["logits"], "softmax2_argmax", 0), (mr_batch, "channel", 1), (mr_batch_y, "argmax", 0)])
+                writers[log_dir].add_images([(tag, u8[s, i]) for s, name in enumerate(self.TRAIN_IMAGE_TAGS)
+                                             for i, tag in enumerate(image_tags(name, u8.shape[1]))], step)
             writers[log_dir].flush()
             with open(os.path.join(log_dir, "scalars.jsonl"), "a") as f:
                 f.write(json.dumps(dict(step=int(step), **scalars)) + "\n")
@@ -676,7 +690,9 @@ class Trainer(object):
         return sum(float(t.detach()) * w for t, w in terms)
 
     # ---- schedule (adversarial.py:767-940) ---------------------------------------------------------------------------------
-    def train(self, output_path, restore=True, restored_path=None, training_iters=200, epochs=1000, dropout=0.75, display_step=5):
+    def train(self, output_path, restore=True, restored_path=None, training_iters=200, epochs=1000, dropout=0.75, display_step=5,
+              image_summaries=False):
+        """adversarial.py:767-946; `image_summaries` also writes both monitoring passes' image summaries (TRAIN_IMAGE_TAGS)"""
         save_path = os.path.join(output_path, "model.cpkt")
         if epochs == 0:
             return save_path
@@ -718,6 +734,7 @@ class Trainer(object):
         upd_interval = cfg.get("iter_upd_interval", 999999999999)
         ckpt_space = cfg.get("checkpoint_space", 100)
         decay = cfg.get("lr_decay_factor", 0.98)
+        img = {"image_summaries": True} if image_summaries else {}       # the monitoring calls stay as they were when off
         for epoch in range(epochs):
             for step in range(epoch * training_iters, (epoch + 1) * training_iters):
                 start = time.time()
@@ -740,7 +757,7 @@ class Trainer(object):
                     for sub, detail, cs, ms in (("train_log", False, ct_src, mr_src), ("val_log", True, ct_val, mr_val)):
                         (ct, cty), (mr, mry) = cs.next(), ms.next()
                         self.output_minibatch_stats(step, to_device(ct, dev), to_device(cty, dev), to_device(mr, dev), to_device(mry, dev),
-                                                    os.path.join(output_path, sub + tag), detail)
+                                                    os.path.join(output_path, sub + tag), detail, **img)
                 if step % ckpt_space == 0 and step != 0:
                     self.save(save_path, output_path)
                     # "Model has been restored for re-allocation" (adversarial.py:929-935): the reference re-reads the checkpoint it

@@ -762,13 +762,94 @@ logits_argmax_concat_kernel(const float* __restrict__ logits, float* __restrict_
 // ------------------------------------------------------------------------------------------------
 constexpr int kMaxC = 8;
 
+// pixel_wise_softmax_2 (layers.py:134-138) of one pixel's C <= kMaxC logits l[] into o[]; shared by pixel_softmax2_kernel and the
+// image summaries' compact prediction, so both see the same values bit for bit
+__device__ __forceinline__ void pixel_softmax2_px(const float* __restrict__ l, float* __restrict__ o, int C) {
+  float e[kMaxC], s = 0.f;
+  for (int c = 0; c < C; ++c) { e[c] = expf(l[c]); s += e[c]; }   // no max subtraction (layers.py:135)
+  for (int c = 0; c < C; ++c) o[c] = fminf(fmaxf(e[c] / s, -1e15f), 1e15f);
+}
+
 __global__ void __launch_bounds__(256)
 pixel_softmax2_kernel(const float* __restrict__ logits, float* __restrict__ out, long long P, int C) {
   pnp_pdl_enter();
-  for (long long p = (long long)blockIdx.x * 256 + threadIdx.x; p < P; p += (long long)gridDim.x * 256) {
-    float e[kMaxC], s = 0.f;
-    for (int c = 0; c < C; ++c) { e[c] = expf(logits[p * C + c]); s += e[c]; }   // no max subtraction (layers.py:135)
-    for (int c = 0; c < C; ++c) out[p * C + c] = fminf(fmaxf(e[c] / s, -1e15f), 1e15f);
+  for (long long p = (long long)blockIdx.x * 256 + threadIdx.x; p < P; p += (long long)gridDim.x * 256)
+    pixel_softmax2_px(logits + p * C, out + p * C, C);
+}
+
+// ---- tf.summary.image panels (TF-1.4 ImageSummaryOp, float path) --------------------------------------------------------------
+constexpr int kImgMaxSrc = 6;
+constexpr int kImgThreads = 512;
+
+struct ImgPlan {
+  const float* src[kImgMaxSrc];
+  int kind[kImgMaxSrc];     // PNP_IMG_CHANNEL / PNP_IMG_ARGMAX / PNP_IMG_SOFTMAX2_ARGMAX
+  int C[kImgMaxSrc];
+  int ch[kImgMaxSrc];
+};
+
+// the single-channel value pixel p of a panel shows: channel `ch`, or the first-max class index (tf.argmax) of the C channels or
+// of their pixel_wise_softmax_2 values
+__device__ __forceinline__ float img_value(const float* __restrict__ x, long long p, int kind, int C, int ch) {
+  const float* px = x + p * C;
+  if (kind == PNP_IMG_CHANNEL) return px[ch];
+  float v[kMaxC];
+  if (kind == PNP_IMG_SOFTMAX2_ARGMAX) pixel_softmax2_px(px, v, C);
+  else
+    for (int c = 0; c < C; ++c) v[c] = px[c];
+  int arg = 0;
+  float best = v[0];
+  for (int c = 1; c < C; ++c)
+    if (v[c] > best) { best = v[c]; arg = c; }
+  return (float)arg;
+}
+
+// One CTA per (source, image) panel.  NormalizeFloatImage of summary_image_op.cc: min / max over the finite pixels (a block-wide
+// fmin / fmax, order-independent, so exact), then scale = 127 / max|.| with offset 128 if the min is negative, else 255 / max with
+// offset 0 (scale 0 below 1e-6), pixel = uint8(trunc(v * scale + offset)), a non-finite pixel = bad_color[0] = 255.  The product and
+// the sum are rounded separately (nvcc would contract them into an FMA); whether TensorFlow's own CPU build contracted them
+// depends on its compiler flags and cannot be recovered, so the uncontracted form as written in the source is what is computed.
+__global__ void __launch_bounds__(kImgThreads)
+image_summary_u8_kernel(ImgPlan plan, int n, long long HW, unsigned char* __restrict__ out) {
+  pnp_pdl_enter();
+  __shared__ float s_mn[kImgThreads / 32], s_mx[kImgThreads / 32];
+  __shared__ float s_scale, s_offset;
+  const int s = blockIdx.x / n, i = blockIdx.x % n;
+  const int kind = plan.kind[s], C = plan.C[s], ch = plan.ch[s];
+  const float* x = plan.src[s] + (long long)i * HW * C;
+  float mn = INFINITY, mx = -INFINITY;
+  for (long long p = threadIdx.x; p < HW; p += kImgThreads) {
+    const float v = img_value(x, p, kind, C, ch);
+    if (isfinite(v)) { mn = fminf(mn, v); mx = fmaxf(mx, v); }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
+  if ((threadIdx.x & 31) == 0) { s_mn[threadIdx.x >> 5] = mn; s_mx[threadIdx.x >> 5] = mx; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < kImgThreads / 32; ++w) { mn = fminf(mn, s_mn[w]); mx = fmaxf(mx, s_mx[w]); }
+    const float kZeroThreshold = 1e-6f;
+    float scale, offset;
+    if (mn < 0.f) {
+      const float max_val = fmaxf(fabsf(mn), fabsf(mx));
+      scale = max_val < kZeroThreshold ? 0.f : __fdiv_rn(127.f, max_val);
+      offset = 128.f;
+    } else {
+      scale = mx < kZeroThreshold ? 0.f : __fdiv_rn(255.f, mx);
+      offset = 0.f;
+    }
+    s_scale = scale;
+    s_offset = offset;
+  }
+  __syncthreads();
+  const float scale = s_scale, offset = s_offset;
+  unsigned char* o = out + (long long)blockIdx.x * HW;
+  for (long long p = threadIdx.x; p < HW; p += kImgThreads) {
+    const float v = img_value(x, p, kind, C, ch);
+    o[p] = isfinite(v) ? (unsigned char)__float2uint_rz(__fadd_rn(__fmul_rn(v, scale), offset)) : (unsigned char)255;
   }
 }
 
@@ -1375,6 +1456,28 @@ extern "C" int pnp_pixel_softmax2(const float* logits, float* out, long long P, 
   if (!logits || !out || P <= 0 || C <= 0) return PNP_ERR_BAD_ARG;
   if (C > kMaxC) return PNP_ERR_UNSUPPORTED;
   pnp_launch(pixel_softmax2_kernel, grid_for(P, 256 * 2), 256, 0, S_, logits, out, P, C);
+  PNP_LAUNCH_CHECK();
+  return PNP_OK;
+}
+
+extern "C" int pnp_image_summary_u8(const float* const* srcs, const int* kinds, const int* C, const int* channel, int nsrc,
+                                    int B, int H, int W, int n, unsigned char* out, void* stream) {
+  if (!srcs || !kinds || !C || !channel || !out || nsrc < 1 || B <= 0 || H <= 0 || W <= 0 || n < 1 || n > B) return PNP_ERR_BAD_ARG;
+  if (nsrc > kImgMaxSrc) return PNP_ERR_UNSUPPORTED;
+  ImgPlan plan;
+  for (int s = 0; s < kImgMaxSrc; ++s) { plan.src[s] = nullptr; plan.kind[s] = plan.C[s] = plan.ch[s] = 0; }
+  for (int s = 0; s < nsrc; ++s) {
+    if (!srcs[s] || C[s] <= 0) return PNP_ERR_BAD_ARG;
+    if (kinds[s] == PNP_IMG_CHANNEL) {
+      if (channel[s] < 0 || channel[s] >= C[s]) return PNP_ERR_BAD_ARG;
+    } else if (kinds[s] == PNP_IMG_ARGMAX || kinds[s] == PNP_IMG_SOFTMAX2_ARGMAX) {
+      if (C[s] > kMaxC) return PNP_ERR_UNSUPPORTED;
+    } else {
+      return PNP_ERR_BAD_ARG;
+    }
+    plan.src[s] = srcs[s]; plan.kind[s] = kinds[s]; plan.C[s] = C[s]; plan.ch[s] = channel[s];
+  }
+  pnp_launch(image_summary_u8_kernel, (unsigned)(nsrc * n), kImgThreads, 0, S_, plan, n, (long long)H * W, out);
   PNP_LAUNCH_CHECK();
   return PNP_OK;
 }

@@ -970,6 +970,31 @@ def pixel_softmax2(logits):
     return out
 
 
+IMG_KINDS = {"channel": 0, "argmax": 1, "softmax2_argmax": 2}       # PNP_IMG_* of include/pnp_b200.h
+
+
+def image_summary(sources, max_outputs=3):
+    """The uint8 panels of tf.summary.image(name, tf.expand_dims(tf.cast(t, tf.float32), 3), max_outputs) for every source of
+    one monitoring pass, in one launch and one device->host copy.  `sources`: list of (tensor fp32 [B,H,W,C] on the device, kind,
+    channel) with kind "channel" (t = tensor[..., channel]), "argmax" (t = tf.argmax(tensor, 3)) or "softmax2_argmax"
+    (t = tf.argmax(pixel_wise_softmax_2(tensor), 3)); every source has the same B, H, W.
+    Returns a host numpy.uint8 array [nsrc, min(B, max_outputs), H, W]."""
+    ts = [t.contiguous() for t, _, _ in sources]
+    B, H, W = ts[0].shape[:3]
+    for t in ts:
+        if t.dim() != 4 or tuple(t.shape[:3]) != (B, H, W) or t.dtype != torch.float32:
+            raise ValueError("image_summary: every source must be fp32 [%d, %d, %d, C], got %s %s" % (B, H, W, tuple(t.shape), t.dtype))
+    n, ns = min(B, int(max_outputs)), len(ts)
+    dev = torch.empty(ns, n, H, W, dtype=torch.uint8, device=ts[0].device)
+    ia = lambda vals: (ctypes.c_int * ns)(*vals)
+    call("pnp_image_summary_u8", (ctypes.c_void_p * ns)(*[t.data_ptr() for t in ts]), ia([IMG_KINDS[k] for _, k, _ in sources]),
+         ia([t.shape[3] for t in ts]), ia([int(c) for _, _, c in sources]), ns, B, H, W, n, ptr(dev), rt.stream())
+    host = torch.empty(dev.shape, dtype=torch.uint8, pin_memory=True)
+    host.copy_(dev, non_blocking=True)
+    torch.cuda.current_stream().synchronize()
+    return host.numpy()
+
+
 def one_hot(labels, num_cls):
     """device-side lib._label_decomp (lib.py:75-92): int64 [..] -> fp32 [.., num_cls]"""
     labels = labels.contiguous().to(torch.int64)

@@ -231,6 +231,10 @@ class Trainer(object):
     # scalar tags of the merged summary op, in its order (source_segmenter.py:387-396)
     SCALAR_TAGS = ("loss", "regularizer_loss", "weighted_loss", "dice_loss", "dice_eval", "dice_eval_c1", "dice_eval_c2", "dice_eval_c3",
                    "dice_eval_c4")
+    # image summaries of the two merged image ops, in their order (source_segmenter.py:398-405): [compact_pred, x[:,:,:,1], compact_y].
+    # The validation list's 'image' is the graph's second summary of that name, so its name scope (= tag) is uniquified to 'image_1'
+    TRAIN_IMAGE_TAGS = ("train_pred", "image", "GND")
+    VAL_IMAGE_TAGS = ("val_pred", "image_1", "validation_GND")
 
     def _scalars(self, logits, batch_y, wce, dice):
         d, arr = self.net.dice_eval(logits, batch_y)
@@ -238,9 +242,10 @@ class Trainer(object):
                [float(arr[i]) for i in range(1, 5)]
         return dict(zip(self.SCALAR_TAGS, vals))
 
-    def _write_scalars(self, log_dir, step, scalars):
+    def _write_scalars(self, log_dir, step, scalars, images=None):
         """tf.summary.FileWriter(output_path + '/train_log' | '/val_log').add_summary(scalar_summary_op, step) (source_segmenter.py:
-        464-465, 537-539, 567-569): a TensorBoard event file plus the same numbers as one JSON line; rank 0 only"""
+        464-465, 537-539, 567-569): a TensorBoard event file plus the same numbers as one JSON line; rank 0 only.  `images`
+        (tag, uint8 panel) pairs follow as a second event with the same step, as add_summary(summary_img, step) does"""
         if log_dir is None or self.dp.rank != 0:
             return
         import json
@@ -249,20 +254,33 @@ class Trainer(object):
         if log_dir not in writers:
             writers[log_dir] = FileWriter(log_dir)
         writers[log_dir].add_scalars(scalars, step)
+        if images is not None:
+            writers[log_dir].add_images(images, step)
         writers[log_dir].flush()
         with open(os.path.join(log_dir, "scalars.jsonl"), "a") as f:
             f.write(json.dumps(dict(step=int(step), **scalars)) + "\n")
 
-    def output_minibatch_stats(self, batch_x, batch_y, step=None, log_dir=None):
+    def _images(self, log_dir, names, logits, batch_x, batch_y):
+        """the panels of one merged image op from the pass's own tensors -- [compact_pred, x[:,:,:,1], compact_y] -- as
+        (tag, uint8 [H, W]) pairs in the merged op's order; None where nothing is written (no log_dir, or not rank 0)"""
+        if log_dir is None or self.dp.rank != 0:
+            return None
+        from .summary import image_tags
+        u8 = F.image_summary([(logits, "softmax2_argmax", 0), (batch_x, "channel", 1), (batch_y, "argmax", 0)])
+        return [(tag, u8[s, i]) for s, name in enumerate(names) for i, tag in enumerate(image_tags(name, u8.shape[1]))]
+
+    def output_minibatch_stats(self, batch_x, batch_y, step=None, log_dir=None, image_summaries=False):
         """source_segmenter.py:525-539: the tensorboard pass on the training batch feeds x, y and keep_prob 1 ONLY -- both BN
         switches stay at their placeholder default True, so this forward runs batch-statistics BN and (updates_collections=None)
         moves the moving averages once more.  Reproduced because it changes the trained model's moving statistics.  With `log_dir`
-        the nine scalar summaries of the reference go to an event file there."""
+        the nine scalar summaries of the reference go to an event file there; `image_summaries` adds the TRAIN_IMAGE_TAGS panels
+        of this forward as a second event with the same step."""
         with torch.no_grad():
             logits = self.net.forward(batch_x, keep_prob=1.0, main_bn=True, adapt_bn=True)
             wce, dice = self.net.losses(logits, batch_y)
             if log_dir is not None:
-                self._write_scalars(log_dir, step, self._scalars(logits, batch_y, wce, dice))
+                images = self._images(log_dir, self.TRAIN_IMAGE_TAGS, logits, batch_x, batch_y) if image_summaries else None
+                self._write_scalars(log_dir, step, self._scalars(logits, batch_y, wce, dice), images)
         return self.net.cost_value(wce, dice)
 
     def feed(self, images, raw_labels):
@@ -272,9 +290,11 @@ class Trainer(object):
         y = _label_decomp(self.num_cls, to_device(raw_labels, dev))
         return x, y
 
-    def train(self, output_path, restored_path=None, restore=False, training_iters=100, epochs=100, display_step=5, dropout=0.75):
+    def train(self, output_path, restored_path=None, restore=False, training_iters=100, epochs=100, display_step=5, dropout=0.75,
+              image_summaries=False):
         """source_segmenter.py:429-525: optimizer steps, the two monitoring passes every `display_step` (training batch with batch-statistics
-        BN, then a validation batch in inference mode) with their scalar summaries, checkpoint + LR*0.9."""
+        BN, then a validation batch in inference mode) with their scalar summaries, checkpoint + LR*0.9.  `image_summaries` also
+        writes each pass's image summaries (TRAIN_IMAGE_TAGS / VAL_IMAGE_TAGS) after its scalars."""
         save_path = os.path.join(output_path, "model.cpkt")
         if epochs == 0:
             return save_path
@@ -314,6 +334,7 @@ class Trainer(object):
             val_src = TFRecordSource(self.val_list, self.batch_size, seed=4321 + self.dp.rank)
         else:
             val_src = SyntheticSource(self.batch_size, seed=4321 + self.dp.rank, num_cls=self.num_cls)
+        img = {"image_summaries": True} if image_summaries else {}       # the monitoring calls stay as they were when off
         for epoch in range(epochs):
             for step in range(epoch * training_iters, (epoch + 1) * training_iters):
                 start = time.time()
@@ -321,12 +342,12 @@ class Trainer(object):
                 x, y = self.feed(images, raw_y)
                 wce, dice = self.train_step(x, y, dropout)
                 if step % display_step == 0:
-                    loss = self.output_minibatch_stats(x, y, step, os.path.join(output_path, "train_log"))
+                    loss = self.output_minibatch_stats(x, y, step, os.path.join(output_path, "train_log"), **img)
                     logging.info("Training at step %s epoch %s , loss is %0.4f" % (step, epoch, loss))
                     logging.info("Time elapsed %s seconds" % (time.time() - start))
                     # source_segmenter.py:498-505: a validation batch right after it, always with the per-organ table
                     vx, vy = self.feed(*val_src.next())
-                    self.val_stats(vx, vy, step, os.path.join(output_path, "val_log"), detail=True)
+                    self.val_stats(vx, vy, step, os.path.join(output_path, "val_log"), detail=True, **img)
                 if step % self.checkpoint_space == 0 and step > 10000:
                     self.save(save_path, output_path)
                     self.optimizer.set_lr(self.optimizer.get_lr() * 0.9)
@@ -347,9 +368,10 @@ class Trainer(object):
             _save(st, os.path.join(output_path, "latest"))
         self.dp.save_checkpoint(write)
 
-    def val_stats(self, batch_x, batch_y, step=None, log_dir=None, detail=False):
+    def val_stats(self, batch_x, batch_y, step=None, log_dir=None, detail=False, image_summaries=False):
         """source_segmenter.py:541-570: inference-mode forward (BN moving stats, keep_prob 1) on a validation batch; `detail` prints
-        the per-organ Dice / Jaccard table of the batch's confusion matrix; with `log_dir` the scalar summaries go to an event file"""
+        the per-organ Dice / Jaccard table of the batch's confusion matrix; with `log_dir` the scalar summaries go to an event file,
+        followed by the VAL_IMAGE_TAGS panels of this forward if `image_summaries`"""
         from .lib import _indicator_eval
         with torch.no_grad():
             logits = self.net.forward(batch_x, keep_prob=1.0, main_bn=False, adapt_bn=False)
@@ -358,7 +380,8 @@ class Trainer(object):
             if detail:
                 _indicator_eval(self.net.confusion_matrix(logits, batch_y).cpu().numpy())
             if log_dir is not None:
-                self._write_scalars(log_dir, step, self._scalars(logits, batch_y, wce, dice))
+                images = self._images(log_dir, self.VAL_IMAGE_TAGS, logits, batch_x, batch_y) if image_summaries else None
+                self._write_scalars(log_dir, step, self._scalars(logits, batch_y, wce, dice), images)
         return {"loss": self.net.cost_value(wce, dice), "dice_eval": float(d), "dice_arr": [float(a) for a in arr]}
 
     # ---- test protocol on NIfTI subjects (source_segmenter.py:572-675) -----------------------------------------------

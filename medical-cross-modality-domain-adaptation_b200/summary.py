@@ -1,19 +1,24 @@
-"""TensorBoard event files without TensorFlow: what `tf.summary.FileWriter(dir)` + `add_summary(scalar_summary_op, step)` leave on
-disk (adversarial.py:664-697, 807-808, 989-991; source_segmenter.py:394-407, 452-453, 537-539).
+"""TensorBoard event files without TensorFlow: what `tf.summary.FileWriter(dir)` + `add_summary(scalar_summary_op, step)` +
+`add_summary(image_summary_op, step)` leave on disk (adversarial.py:664-697, 807-808, 989-991; source_segmenter.py:394-409,
+452-453, 537-539, 568-570).
 
 An event file is a TFRecord stream (the framing `tfrecord.write_record` already implements: u64 length, masked CRC32C of the length,
-payload, masked CRC32C of the payload -- CRC32C from libpnp_io.so) of serialized `tensorflow.Event` messages.  Only four fields are
-needed and they are encoded by hand from event.proto / summary.proto:
+payload, masked CRC32C of the payload -- CRC32C from libpnp_io.so) of serialized `tensorflow.Event` messages.  The fields needed
+are encoded by hand from event.proto / summary.proto:
 
     Event   { double wall_time = 1; int64 step = 2; oneof what { string file_version = 3; Summary summary = 5; } }
-    Summary { repeated Value value = 1; }      Value { string tag = 1; float simple_value = 2; }
+    Summary { repeated Value value = 1; }      Value { string tag = 1; float simple_value = 2; Image image = 4; }
+    Image   { int32 height = 1; int32 width = 2; int32 colorspace = 3; bytes encoded_image_string = 4; }
 
-The first record of a file is the version event `brain.Event:2`, as TensorFlow writes it.  Image summaries (`tf.summary.image`) are
-not written (SURVEY 2.1: out of scope).  tests/test_summary_cpu.py reads the files back with the `tensorboard` package's own loader."""
+The first record of a file is the version event `brain.Event:2`, as TensorFlow writes it.  Image summaries carry 8-bit grayscale
+PNGs (`encode_png`, stdlib zlib) of the uint8 panels that functional.image_summary renders on the GPU, tagged as TF-1.4's
+ImageSummaryOp tags them (`image_tags`).  The `graph=sess.graph` GraphDef event is not written.  tests/test_summary_cpu.py and
+tests/test_image_summary_cpu.py read the files back with the `tensorboard` package's own loader."""
 import os
 import socket
 import struct
 import time
+import zlib
 
 from .tfrecord import _enc_varint, _ld, masked_crc
 
@@ -28,6 +33,41 @@ def encode_scalar_summary(scalars):
     for tag, v in scalars:
         value = _ld(1, str(tag).encode("utf-8")) + _key(2, 5) + struct.pack("<f", float(v))
         out += _ld(1, value)
+    return out
+
+
+def _png_chunk(kind, data):
+    return struct.pack(">I", len(data)) + kind + data + struct.pack(">I", zlib.crc32(kind + data) & 0xFFFFFFFF)
+
+
+def encode_png(u8_hw):
+    """8-bit grayscale PNG (colour type 0) of a uint8 [H, W] array: every row with filter byte 0 (none), one IDAT deflated at
+    zlib's default level (TF's png encoder runs with compression = -1, the same default)"""
+    import numpy as np
+    a = np.ascontiguousarray(u8_hw, dtype=np.uint8)
+    if a.ndim != 2 or a.shape[0] < 1 or a.shape[1] < 1:
+        raise ValueError("encode_png: expected a non-empty uint8 [H, W] array, got shape %s" % (a.shape,))
+    h, w = a.shape
+    raw = np.zeros((h, w + 1), np.uint8)
+    raw[:, 1:] = a
+    ihdr = struct.pack(">IIBBBBB", w, h, 8, 0, 0, 0, 0)
+    return (b"\x89PNG\r\n\x1a\n" + _png_chunk(b"IHDR", ihdr) + _png_chunk(b"IDAT", zlib.compress(raw.tobytes(), -1))
+            + _png_chunk(b"IEND", b""))
+
+
+def image_tags(name, n):
+    """the tags TF-1.4's ImageSummaryOp gives the first n images of a batch when max_images > 1: '<name>/image/<i>'"""
+    return ["%s/image/%d" % (name, i) for i in range(n)]
+
+
+def encode_image_summary(images):
+    """Summary message with one Value{tag, image} per (tag, uint8 [H, W] panel) pair, in the given order (colorspace 1 = depth 1)"""
+    out = b""
+    for tag, u8 in images:
+        h, w = u8.shape
+        img = (_key(1, 0) + _enc_varint(int(h)) + _key(2, 0) + _enc_varint(int(w)) + _key(3, 0) + _enc_varint(1)
+               + _ld(4, encode_png(u8)))
+        out += _ld(1, _ld(1, str(tag).encode("utf-8")) + _ld(4, img))
     return out
 
 
@@ -48,7 +88,7 @@ def frame(payload):
 
 
 class FileWriter(object):
-    """tf.summary.FileWriter for scalars: `events.out.tfevents.<seconds>.<hostname>` under `logdir`, appended and flushed per call."""
+    """tf.summary.FileWriter for scalar and image summaries: `events.out.tfevents.<seconds>.<hostname>` under `logdir`, appended and flushed per call."""
 
     def __init__(self, logdir, filename_suffix=""):
         os.makedirs(logdir, exist_ok=True)
@@ -65,6 +105,11 @@ class FileWriter(object):
         `scalars`: dict (insertion order kept) or a list of pairs."""
         items = list(scalars.items()) if hasattr(scalars, "items") else list(scalars)
         ev = encode_event(time.time() if wall_time is None else wall_time, step=step, summary=encode_scalar_summary(items))
+        self._f.write(frame(ev))
+
+    def add_images(self, images, step, wall_time=None):
+        """one Event carrying every (tag, uint8 [H, W] panel) pair: add_summary(sess.run(tf.summary.merge(image_summaries)), step)"""
+        ev = encode_event(time.time() if wall_time is None else wall_time, step=step, summary=encode_image_summary(list(images)))
         self._f.write(frame(ev))
 
     def add_summary(self, summary, global_step=None):

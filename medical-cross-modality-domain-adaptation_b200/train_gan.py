@@ -64,6 +64,8 @@ def main(phase, argv=None):
     ap.add_argument("--conv-backend", default=None, choices=["auto", "simt", "tc3", "tc1"])
     ap.add_argument("--lists", default="./lists", help="directory of mr_train_list, mr_val_list, ct_train_list, ct_val_list")
     ap.add_argument("--synthetic", action="store_true", help="ignore the list files and train on the synthetic sources")
+    ap.add_argument("--image-summaries", action="store_true",
+                    help="also write the reference's TensorBoard image summaries (prediction, input slice, ground truth) every display step")
     a = ap.parse_args(argv)
     logging.basicConfig(level=logging.INFO)
     parallel.init_from_env()
@@ -83,4 +85,4 @@ def main(phase, argv=None):
                           opt_kwargs=dict(opt_kwargs), train_config=tc)
     print("Now start training...")
     return trainer.train(output_path=out, restored_path=out, training_iters=a.training_iters or tc["training_iters"],
-                         epochs=a.epochs or tc["epochs"], dropout=a.keep_prob)
+                         epochs=a.epochs or tc["epochs"], dropout=a.keep_prob, image_summaries=a.image_summaries)

@@ -54,6 +54,8 @@ def main(argv=None):
     ap.add_argument("--train-list", default=train_fid)
     ap.add_argument("--val-list", default=val_fid)
     ap.add_argument("--synthetic", action="store_true", help="ignore the list files and train on the synthetic source")
+    ap.add_argument("--image-summaries", action="store_true",
+                    help="also write the reference's TensorBoard image summaries (prediction, input slice, ground truth) every display step")
     a = ap.parse_args(argv)
     logging.basicConfig(level=logging.INFO)
     parallel.init_from_env()
@@ -66,7 +68,7 @@ def main(argv=None):
                           checkpoint_space=checkpoint_space, optimizer=optimizer, lr_update_flag=False)
     print("Now start training...")
     return trainer.train(output_path=a.output_path, restored_path=a.output_path, training_iters=a.training_iters,
-                         epochs=a.epochs, restore=restore, dropout=a.keep_prob)
+                         epochs=a.epochs, restore=restore, dropout=a.keep_prob, image_summaries=a.image_summaries)
 
 
 if __name__ == "__main__":
