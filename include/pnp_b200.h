@@ -137,7 +137,10 @@ int pnp_conv2d_tc_wgrad(const uint16_t* x_hi, const uint16_t* x_lo, const uint16
  * replaces tf.contrib.layers.batch_norm(decay .9, eps 1e-3) (layers.py:95-100), the activation
  * (layers.py:12-14) and the residual add with channel-pad skip (layers.py:160-166,182-189). */
 int pnp_bn_stats(const float* z, long long M, int C, double* sum, double* sumsq, void* stream);
-/* training != 0: batch statistics (biased var), moving stats <- 0.9*moving + 0.1*(mean, unbiased var)
+/* training != 0: batch statistics (biased var), moving stats <- 0.9*moving + 0.1*(mean, unbiased var).  The variance is one-pass,
+ * var = sumsq/M - mean^2 from pnp_bn_stats' fp32 partial sums (64 rows per thread, then fp64): its error is bounded by a small
+ * multiple of 2^-24 * E[z^2], not of var, so the relative error of invstd grows as (mean/std)^2 (DESIGN 4.4).  invstd is within
+ * 2 fp32 ulps of the correctly rounded 1/sqrt(fl(var + eps)).
  * training == 0: moving statistics.  Writes scale=gamma*invstd, shift=beta-mean*scale, mean, invstd. */
 int pnp_bn_finalize(const double* sum, const double* sumsq, long long M, int C, const float* gamma,
                     const float* beta, float* moving_mean, float* moving_var, int training,
@@ -158,6 +161,8 @@ int pnp_bn_bwd_apply_fused(const float* g, const float* z, const float* mean, co
 /* The same backward pass WITHOUT the fp32 g = dy*act'(y) round trip (layers whose g nobody else needs, i.e. no residual skip
  * hanging off them): pnp_bn_bwd_reduce_sums accumulates sum(g), sum(g*xhat) only; pnp_bn_bwd_apply_direct recomputes g from dy.
  * The activation sign may come from the bf16 hi plane of y (y_hi) instead of y; dz may be NULL when only the planes are wanted.
+ * The two agree for every y an activation of this library writes (pnp_bn_act_apply, pnp_bn_apply_fused, the fused wgmma
+ * epilogue): those flush positive subnormal activations to +0, since rn_bf16 sends 0 < y <= 2^-134 to +0.
  * 24-28 instead of 32 bytes per element. */
 int pnp_bn_bwd_reduce_sums(const float* dy, const float* y, const uint16_t* y_hi, const float* z, const float* mean,
                            const float* invstd, int act, double* sum_g, double* sum_gx, long long M, int C, void* stream);
@@ -165,7 +170,8 @@ int pnp_bn_bwd_apply_direct(const float* dy, const float* y, const uint16_t* y_h
                             const float* invstd, const float* gamma, const double* sum_g, const double* sum_gx, long long M, int C,
                             int training, const pnp_dropout_cfg* drop, float* dgamma, float* dbeta, float* dz, uint16_t* dz_hi,
                             uint16_t* dz_lo, void* stream);
-/* y = act(z*scale + shift + skip);  skip (optional) has Cs channels placed at channel offset skip_off.
+/* y = act(z*scale + shift + skip);  skip (optional) has Cs channels placed at channel offset skip_off.  ReLU and leaky ReLU
+ * write positive subnormal results as +0 (here, in pnp_bn_apply_fused and in the wgmma fused epilogue).
  * y_hi / y_lo (optional): also emit the bf16 (hi, lo) operand planes of y for the next tensor-core convolution */
 int pnp_bn_act_apply(const float* z, const float* scale, const float* shift, const float* skip, int Cs,
                      int skip_off, int act, float* y, uint16_t* y_hi, uint16_t* y_lo, long long M, int C, void* stream);

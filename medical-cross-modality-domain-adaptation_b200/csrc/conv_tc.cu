@@ -544,10 +544,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
           const float2 sk = __ldg(reinterpret_cast<const float2*>(a.ep_skip + pix[h] * a.ep_skip_c - a.ep_skip_off + ch));
           o.x += sk.x; o.y += sk.y;
         }
+        // positive subnormals go to +0, as in elementwise.cu act_fwd: the hi plane of y then carries the sign of y exactly
+        // (rn_bf16 sends 0 < y <= 2^-134 to +0), which the backward kernels read instead of y
+        constexpr float kMinNormal = 1.17549435e-38f;   // FLT_MIN
         if (a.ep_act == PNP_ACT_RELU) {
-          o.x = o.x > 0.f ? o.x : 0.f; o.y = o.y > 0.f ? o.y : 0.f;
+          o.x = o.x >= kMinNormal ? o.x : 0.f; o.y = o.y >= kMinNormal ? o.y : 0.f;
         } else if (a.ep_act == PNP_ACT_LRELU) {
-          o.x = o.x > 0.f ? o.x : 0.2f * o.x; o.y = o.y > 0.f ? o.y : 0.2f * o.y;
+          o.x = o.x >= kMinNormal ? o.x : (o.x > 0.f ? 0.f : 0.2f * o.x);
+          o.y = o.y >= kMinNormal ? o.y : (o.y > 0.f ? 0.f : 0.2f * o.y);
         }
         const long long e0 = pix[h] * a.Cout + ch;   // flat element index of this thread's pair
         if (out != nullptr) {

@@ -29,9 +29,13 @@ constexpr float kLeak = 0.2f;       // tf.nn.leaky_relu default alpha (layers.py
 constexpr float kBnDecay = 0.90f;   // layers.py:100
 constexpr float kBnEps = 1e-3f;     // tf.contrib.layers.batch_norm default epsilon
 
+constexpr float kMinNormal = 1.17549435e-38f;   // FLT_MIN = 2^-126
+
+// Positive subnormal activations are flushed to +0: round-to-nearest sends 0 < y <= 2^-134 to a bf16 +0, and the backward
+// kernels may read the sign of y from its hi plane (act_slope), so every y written here satisfies (y > 0) <=> (hi > 0).
 __device__ __forceinline__ float act_fwd(float v, int act) {
-  if (act == PNP_ACT_RELU) return v > 0.f ? v : 0.f;
-  if (act == PNP_ACT_LRELU) return v > 0.f ? v : kLeak * v;
+  if (act == PNP_ACT_RELU) return v >= kMinNormal ? v : 0.f;
+  if (act == PNP_ACT_LRELU) return v >= kMinNormal ? v : (v > 0.f ? 0.f : kLeak * v);
   return v;
 }
 __device__ __forceinline__ float4 hi4_as_float4(ushort4 h) {
@@ -98,7 +102,7 @@ bn_reduce_kernel(const float* __restrict__ z, const float* __restrict__ dy, cons
         float4 gB = __ldg(reinterpret_cast<const float4*>(dy) + offB);
         if (act != PNP_ACT_NONE) {
           float4 yA, yB;
-          if (yact_hi) {       // the sign of y from its bf16 hi plane (round-to-nearest keeps the sign; y == 0 <=> hi == 0)
+          if (yact_hi) {       // the sign of y from its bf16 hi plane: (y > 0) <=> (hi > 0) for every y act_fwd writes
             yA = hi4_as_float4(__ldg(reinterpret_cast<const ushort4*>(yact_hi) + offA));
             yB = hi4_as_float4(__ldg(reinterpret_cast<const ushort4*>(yact_hi) + offB));
           } else {
