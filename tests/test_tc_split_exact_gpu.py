@@ -21,6 +21,7 @@ import pytest
 import torch
 
 from oracle import bf16_split as S
+from oracle import philox
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -174,15 +175,18 @@ def last_config(_C):
 
 def drop_cfg(_C, keep, stream_id=11, seed=0x1234_5678_9ABC):
     seed_t = torch.tensor([seed], dtype=torch.int64, device=DEV)
-    return _C.DropCfg(seed_t.data_ptr(), stream_id, keep), seed_t
+    cfg = _C.DropCfg(seed_t.data_ptr(), stream_id, keep)
+    cfg.seed_value = seed
+    return cfg, seed_t
 
 
 def drop_mask(_C, rt, cfg, shape):
-    """the multipliers pnp_dropout_apply draws for (seed, stream): dropout of a tensor of ones"""
-    ones = torch.ones(shape, dtype=torch.float32, device=DEV)
-    m = torch.empty_like(ones)
-    _C.call("pnp_dropout_apply", _C.ptr(ones), _C.ptr(m), ones.numel(), ctypes.byref(cfg), rt.stream())
-    return m
+    """the multipliers of (seed, stream, keep) from the independent Philox4x32-10 reference (oracle/philox.py)"""
+    n = 1
+    for s in shape:
+        n *= int(s)
+    m = philox.dropout_mult(cfg.seed_value, cfg.stream, cfg.keep, n)
+    return torch.from_numpy(m).reshape(tuple(shape)).to(DEV)
 
 
 def _f64(t):
