@@ -299,9 +299,11 @@ struct TcCfg {
   static constexpr int STAGE_BYTES = NPLANES * (A_TILE_BYTES + B_TILE_BYTES);
   static constexpr int STAGES_RAW = (200 * 1024) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int STAT_BYTES = 2 * BLOCK_N * 8;                 // per-CTA fp64 BN partial sums of the current n-tile
+  // fp64 BN partial sums of the current n-tile, one [sum | sumsq][BLOCK_N] row per consumer warp (16 KB at BLOCK_N = 128)
+  static constexpr int STAT_BYTES = CONSUMER_WARPS * 2 * BLOCK_N * 8;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAT_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(STAGES >= 2, "pipeline needs two stages");
+  // the ring is sized before the statistics rows: they must fit beside it, never cost it a stage
   static_assert(SMEM_BYTES <= 227 * 1024, "H100 allows 227 KB of shared memory per block");
 };
 
@@ -322,8 +324,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   constexpr int ACC = BLOCK_N / 2;                   // fp32 accumulator registers per thread (m64 x BLOCK_N per warpgroup)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  double* stat = reinterpret_cast<double*>(smem + STAGES * Cfg::STAGE_BYTES);    // [sum | sumsq][BLOCK_N]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(stat + 2 * BLOCK_N);              // [0..S) full, [S..2S) empty
+  double* stat = reinterpret_cast<double*>(smem + STAGES * Cfg::STAGE_BYTES);    // [consumer warp][sum | sumsq][BLOCK_N]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stat + CONSUMER_WARPS * 2 * BLOCK_N);   // [0..S) full, [S..2S) empty
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -341,7 +343,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
     }
     fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < 2 * BLOCK_N; i += TC_THREADS) stat[i] = 0.0;
+  for (int i = threadIdx.x; i < CONSUMER_WARPS * 2 * BLOCK_N; i += TC_THREADS) stat[i] = 0.0;
   __syncthreads();
   pnp_pdl_wait();                             // from here on the predecessor kernel's results are read / its buffers written
 
@@ -389,16 +391,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   const bool drop_on = a.drop.seed_ptr != nullptr;
   unsigned long long seed = 0ull;
   if (drop_on) seed = *a.drop.seed_ptr;
-  // BN partial statistics: warp-reduced, then summed in fp64 in shared memory over every tile of this CTA that shares an
-  // n-tile; one fp64 global atomic per column when the n-tile changes (and at the end), not one per tile
+  // BN partial statistics: warp-reduced in fp32, then summed in fp64 over every tile of this CTA that shares an n-tile, in the
+  // warp's own shared-memory row (one writer per slot: plain adds, no shared-memory atomics, which sm_90 runs as CAS loops on
+  // fp64).  When the n-tile changes (and at the end) the eight rows are summed in a fixed order and each column takes one fp64
+  // global atomic, not one per tile.
+  double* wstat = stat + warp * 2 * BLOCK_N;
   int stat_n0 = -1;
   auto flush_stats = [&]() {
     consumer_sync();
-    for (int i = threadIdx.x; i < BLOCK_N; i += CONSUMER_THREADS) {
-      atomicAdd(a.bn_sum + stat_n0 + i, stat[i]);
-      atomicAdd(a.bn_sumsq + stat_n0 + i, stat[BLOCK_N + i]);
-      stat[i] = 0.0;
-      stat[BLOCK_N + i] = 0.0;
+    for (int i = threadIdx.x; i < 2 * BLOCK_N; i += CONSUMER_THREADS) {
+      double t = 0.0;
+#pragma unroll
+      for (int w = 0; w < CONSUMER_WARPS; ++w) {
+        t += stat[w * 2 * BLOCK_N + i];
+        stat[w * 2 * BLOCK_N + i] = 0.0;
+      }
+      atomicAdd((i < BLOCK_N ? a.bn_sum : a.bn_sumsq) + stat_n0 + (i % BLOCK_N), t);
     }
     consumer_sync();
   };
@@ -522,11 +530,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
           q0 += __shfl_xor_sync(0xffffffffu, q0, off);
           q1 += __shfl_xor_sync(0xffffffffu, q1, off);
         }
-        if (lane < 4) {
-          atomicAdd(stat + c0, (double)s0);
-          atomicAdd(stat + c0 + 1, (double)s1);
-          atomicAdd(stat + BLOCK_N + c0, (double)q0);
-          atomicAdd(stat + BLOCK_N + c0 + 1, (double)q1);
+        // lanes q, q + 4, .., q + 28 now hold the same four sums of columns c0, c0 + 1; lane 4r + q adds the r-th of them
+        if (lane < 16) {
+          const int r = lane >> 2;
+          const float x = r == 0 ? s0 : r == 1 ? s1 : r == 2 ? q0 : q1;
+          wstat[(r >> 1) * BLOCK_N + c0 + (r & 1)] += (double)x;
         }
       }
       float2 sc = make_float2(1.f, 1.f), sh = make_float2(0.f, 0.f);
