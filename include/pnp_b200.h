@@ -292,6 +292,32 @@ int pnp_momentum_step(float* theta, const float* grad, float* accum, long long n
                       const float* lr_ptr, float momentum, float grad_scale, void* stream);
 int pnp_fill(float* p, float v, long long n, void* stream);
 
+/* ---- evaluation: 3-D surface distances ---------------------------------------------------------------------------------------
+ * Per-class surface distances between a predicted label volume P and a ground truth G (medpy.metric.binary.assd / hd as the
+ * papers' evaluation calls them).  pred and gt are uint8 [n0][n1][n2] (n2 fastest) on the device; labels >= C count as
+ * background.  For each class c in 1 .. C-1, with A = (P == c) and B = (G == c):
+ *   dA = A and not erode(A) (6-neighbour cross, one iteration; voxels outside the volume are not in A, so A's voxels on the
+ *   faces of the volume are border voxels), likewise dB;
+ *   d(v, S) = min over s in S of sqrt(((s0 (v0 - s0'))^2 + (s1 (v1 - s1'))^2) + (s2 (v2 - s2'))^2), spacing = (s0, s1, s2);
+ *   out[(c-1)*6 + 0..5] = sum of d(v, dB) over v in dA, |dA|, max of d(v, dB) over dA,
+ *                         sum of d(v, dA) over v in dB, |dB|, max of d(v, dA) over dB   (doubles, device).
+ * If dA or dB is empty the four sums / maxima of that class are NaN (the counts are exact).  ASSD = (out[0]/out[1] +
+ * out[3]/out[4]) / 2, HD = max(out[2], out[5]).  Each distance is exact (an exact Euclidean feature transform, then scipy's
+ * expression above in fp64); with unit spacing it is bit-identical to scipy.ndimage.distance_transform_edt.  The sums run in a
+ * fixed order, so repeated calls give bit-identical results.
+ *
+ * spacing: host pointer to 3 positive finite doubles, or NULL for unit spacing (voxel units).  1 <= n0, n1, n2 <=
+ * PNP_SD_MAX_DIM and 2 <= C <= 8 (one border bit per class in a byte), else PNP_ERR_UNSUPPORTED; non-positive sizes, bad
+ * spacing, NULL pointers or a workspace smaller than pnp_surface_distance_workspace's are PNP_ERR_BAD_ARG.  On any error nothing
+ * is launched and out is untouched.
+ *
+ * Workspace (device, ws_bytes long): with N = n0*n1*n2, L = n1*n2 and A(x) = x rounded up to a multiple of 256,
+ *   bytes = A(2N) + A(4N) + A(8N) + 2 A(16L) + A(8L)      (~14 bytes per voxel: 235 MB at 256^3, for any C). */
+#define PNP_SD_MAX_DIM 1024
+int pnp_surface_distance_workspace(int n0, int n1, int n2, int C, long long* bytes /* host */);
+int pnp_surface_distance(const uint8_t* pred, const uint8_t* gt, int n0, int n1, int n2, int C, const double* spacing /* host, 3 */,
+                         void* ws, long long ws_bytes, double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

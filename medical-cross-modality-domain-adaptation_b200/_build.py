@@ -10,7 +10,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpnp_b200.so")
-SOURCES = ["conv_simt.cu", "elementwise.cu", "conv_tc.cu", "surface.cu"]
+SOURCES = ["conv_simt.cu", "elementwise.cu", "conv_tc.cu", "surface.cu", "metrics3d.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(os.path.dirname(HERE), "include", "pnp_b200.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [ "-O3", "-std=c++17", "-lineinfo",

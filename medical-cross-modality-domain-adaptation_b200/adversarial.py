@@ -535,27 +535,36 @@ class Trainer(object):
                                                          self.num_cls or self.net.n_class, flip_correction, True, rng)
         return dice, jac, cm.astype(np.int64), pred_vol
 
-    def test_eval(self, output_path, flip_correction=True, save_result=False):
+    def test_eval(self, output_path, flip_correction=True, save_result=False, surface_metrics=False):
         """adversarial.py:993-1052: every (label, image) .nii pair of `test_label_list` / `test_nii_list` through the per-subject
         protocol above; writes the summed confusion matrix to <output_path>/cm.csv and returns sample_metric_stddev's pair.
-        `save_result` (the segmenter trainer's switch, source_segmenter.py:625-626) also writes the predictions as .nii.gz."""
+        `save_result` (the segmenter trainer's switch, source_segmenter.py:625-626) also writes the predictions as .nii.gz.
+        `surface_metrics` also scores every subject's prediction by per-organ ASSD / HD on the GPU (evaluation.surface_distances,
+        voxel units), keeps them in `self.sample_surface_list`, prints their mean and spread and writes
+        <output_path>/surface.csv; the return value and the Dice / Jaccard output are unchanged."""
         from . import evaluation
-        sample_eval_list, _ = evaluation.run_test_eval(
-            self._predict_ct, self.test_label_list, self.test_nii_list, self.net.batch_size, self.num_cls or self.net.n_class,
-            output_path, "dense_pred", flip_correction, save_result, shuffle=True, write_cm=True)
-        self.sample_eval_list = sample_eval_list
-        return self.sample_metric_stddev(sample_eval_list)
+        nc = self.num_cls or self.net.n_class
+        res = evaluation.run_test_eval(
+            self._predict_ct, self.test_label_list, self.test_nii_list, self.net.batch_size, nc,
+            output_path, "dense_pred", flip_correction, save_result, shuffle=True, write_cm=True, surface_metrics=surface_metrics)
+        self.sample_eval_list = res[0]
+        out = self.sample_metric_stddev(res[0])
+        if surface_metrics:
+            self.sample_surface_list = res[2]
+            evaluation.surface_metric_stddev(res[2], nc)
+            evaluation.write_surface_csv(os.path.join(output_path, "surface.csv"), res[2], nc)
+        return out
 
     def sample_metric_stddev(self, sample_eval_list):
         """adversarial.py:1054-1084"""
         from . import evaluation
         return evaluation.sample_metric_stddev(sample_eval_list, self.num_cls or self.net.n_class)
 
-    def test_model(self, this_model, output_path):
+    def test_model(self, this_model, output_path, surface_metrics=False):
         """adversarial.py:1097-1108: restore a checkpoint, run the test protocol"""
         self.net.restore(this_model)
         logging.info("model has been loaded!")
-        dice, jac = self.test_eval(output_path)
+        dice, jac = self.test_eval(output_path, surface_metrics=surface_metrics)
         logging.info("testing finished")
         return dice, jac
 

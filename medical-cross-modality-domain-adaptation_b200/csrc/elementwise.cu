@@ -1604,4 +1604,4 @@ extern "C" const char* pnp_error_string(int code) {
   }
 }
 
-extern "C" int pnp_version(void) { return 100; }
+extern "C" int pnp_version(void) { return 101; }

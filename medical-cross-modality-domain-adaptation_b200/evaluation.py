@@ -93,9 +93,75 @@ def eval_volume(predict, raw, raw_y, batch_size, num_cls, flip_correction=True, 
     return _dice(cm), _jaccard(cm), cm, pred_vol
 
 
+SURFACE_COLUMNS = ("assd", "hd", "asd_pred_gt", "asd_gt_pred", "border_pred", "border_gt")
+
+
+def surface_distances(pred_vol, gt_vol, num_cls, spacing=None):
+    """Per-organ surface distances of one subject on the GPU (functional.surface_distances): a dict of [num_cls] arrays `assd`,
+    `hd`, `asd_pred_gt`, `asd_gt_pred` (background and organs absent from either volume: NaN) and the border voxel counts
+    `border_pred`, `border_gt`.  Distances are in voxel units unless `spacing` (three voxel sizes) is given, like SIFA's
+    evaluation.
+
+    `pred_vol` as `eval_volume` / `Trainer.test_eval_volume` return it is in the evaluated orientation: flipped along both
+    in-plane axes when flip_correction is on.  Flip the ground truth the same way before calling, e.g.
+    `surface_distances(pred_vol, np.flip(np.flip(raw_y, 0), 1), num_cls)`.  Frames the protocol never predicts (the first and
+    last, and any a short batch drops) are background in `pred_vol` and are scored as such."""
+    from .functional import surface_distances as _sd
+    return _sd(pred_vol, gt_vol, num_cls, spacing)
+
+
+def _organ_names(num_cls):
+    names = {int(v): k for k, v in contour_map.items()}
+    return [names.get(c, "class_%d" % c) for c in range(num_cls)]
+
+
+def surface_metric_stddev(sample_surface_list, num_cls):
+    """Per-organ spread and mean of ASSD and HD over subjects, printed in the form of sample_metric_stddev's lines.  Subjects where
+    the organ is absent from the prediction or the ground truth (NaN) are left out and counted.  Returns (mean ASSD [num_cls],
+    mean HD [num_cls]), NaN where no subject has the organ in both volumes."""
+    names = _organ_names(num_cls)
+    stats = {}
+    for key in ("assd", "hd"):
+        mat = np.array([s[key] for s in sample_surface_list], np.float64).reshape(len(sample_surface_list), num_cls)
+        stats[key] = [mat[~np.isnan(mat[:, c]), c] for c in range(num_cls)]
+    print("------- surface distances over subjects (voxel units) ---- ")
+    for c in range(1, num_cls):
+        print("organ: %s" % names[c])
+        print("assd_stddev: %s" % (np.std(stats["assd"][c]) if len(stats["assd"][c]) else np.nan))
+        print("hd_stddev: %s" % (np.std(stats["hd"][c]) if len(stats["hd"][c]) else np.nan))
+    print("------- surface distances over subjects (voxel units) ----  ")
+    mean = {k: np.full(num_cls, np.nan) for k in ("assd", "hd")}
+    for c in range(1, num_cls):
+        print("organ: %s" % names[c])
+        for key in ("assd", "hd"):
+            if len(stats[key][c]):
+                mean[key][c] = np.mean(stats[key][c])
+        print("assd_mean: %s" % mean["assd"][c])
+        print("hd_mean: %s" % mean["hd"][c])
+        print("skipped subjects (organ absent from prediction or ground truth): %d" % (len(sample_surface_list) - len(stats["assd"][c])))
+    print("-------")
+    return mean["assd"], mean["hd"]
+
+
+def write_surface_csv(path, sample_surface_list, num_cls):
+    """one row per subject: subject, then <organ>_<column> for every organ and SURFACE_COLUMNS entry (NaN: organ absent)"""
+    names = _organ_names(num_cls)
+    with open(path, "w") as f:
+        f.write(",".join(["subject"] + ["%s_%s" % (names[c], k) for c in range(1, num_cls) for k in SURFACE_COLUMNS]) + "\n")
+        for s in sample_surface_list:
+            row = [str(s["subject"])]
+            for c in range(1, num_cls):
+                row += [str(int(s[k][c])) if k.startswith("border") else repr(float(s[k][c])) for k in SURFACE_COLUMNS]
+            f.write(",".join(row) + "\n")
+    return path
+
+
 def run_test_eval(predict, test_label_list, test_nii_list, batch_size, num_cls, output_path, pred_subdir, flip_correction=True,
-                  save_result=False, shuffle=True, write_cm=False, rng=None):
-    """The subject loop of both `test_eval`s.  Returns (sample_eval_list, summed confusion matrix)."""
+                  save_result=False, shuffle=True, write_cm=False, rng=None, surface_metrics=False):
+    """The subject loop of both `test_eval`s.  Returns (sample_eval_list, summed confusion matrix), and with `surface_metrics`
+    a third value: per subject the dict of `surface_distances` plus its "subject" (the image file's name), computed on the
+    volumes `save_result` writes -- `pred_vol` against the ground truth in the same orientation, labels above the class range
+    as background."""
     pred_folder = os.path.join(output_path, pred_subdir)
     try:
         os.makedirs(pred_folder)
@@ -105,6 +171,7 @@ def run_test_eval(predict, test_label_list, test_nii_list, batch_size, num_cls, 
         raise ValueError("test_eval needs test_label_list and test_nii_list (paths of the label / image .nii files)")
     all_cm = np.zeros([num_cls, num_cls])
     sample_eval_list = []
+    sample_surface_list = []
     for idx_file, (label_fid, nii_fid) in enumerate(zip(test_label_list, test_nii_list)):
         if not os.path.isfile(nii_fid):
             raise Exception("cannot find sample %s" % str(nii_fid))
@@ -114,10 +181,16 @@ def run_test_eval(predict, test_label_list, test_nii_list, batch_size, num_cls, 
         logging.info("sample %d (%s): %d frames processed" % (idx_file, os.path.basename(str(nii_fid)), raw.shape[2]))
         all_cm += cm
         sample_eval_list.append((dice, jac))
+        gth = np.flip(np.flip(np.asarray(raw_y), 0), 1) if flip_correction else np.asarray(raw_y)
         if save_result:
-            gth = np.flip(np.flip(np.asarray(raw_y), 0), 1) if flip_correction else np.asarray(raw_y)
             _save_nii_prediction(gth.astype(np.int16), pred_vol.astype(np.int16), nii_fid, pred_folder,
                                  out_bname="dense_pred_" + os.path.basename(str(nii_fid)), num_cls=num_cls)
+        if surface_metrics:
+            sd = surface_distances(pred_vol.astype(np.int16), gth.astype(np.int16), num_cls)
+            sd["subject"] = os.path.basename(str(nii_fid))
+            sample_surface_list.append(sd)
     if write_cm:
         np.savetxt(os.path.join(output_path, "cm.csv"), all_cm)
+    if surface_metrics:
+        return sample_eval_list, all_cm, sample_surface_list
     return sample_eval_list, all_cm

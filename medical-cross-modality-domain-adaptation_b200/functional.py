@@ -9,6 +9,8 @@ of a flat gradient arena, see optim.py); the Functions return None for them so a
 import ctypes
 import math
 import os
+
+import numpy as np
 import torch
 
 from . import _C
@@ -1001,6 +1003,77 @@ def one_hot(labels, num_cls):
     out = torch.empty(labels.shape + (num_cls,), dtype=torch.float32, device=labels.device)
     call("pnp_one_hot", ptr(labels), ptr(out), labels.numel(), num_cls, rt.stream())
     return out
+
+
+SD_MAX_DIM = 1024        # PNP_SD_MAX_DIM of include/pnp_b200.h
+SURFACE_KEYS = ("asd_pred_gt", "asd_gt_pred", "assd", "hd")
+
+
+def _surface_args(pred, gt, num_cls, spacing):
+    """host-side checks of surface_distances: -> (pred, gt) as uint8 volumes with out-of-range labels mapped to 0, spacing"""
+    num_cls = int(num_cls)
+    if not 2 <= num_cls <= 8:
+        raise ValueError("surface_distances: num_cls must be in [2, 8] (one border bit per class in a byte), got %d" % num_cls)
+    pred, gt = np.asarray(pred), np.asarray(gt)
+    if pred.ndim != 3 or pred.shape != gt.shape:
+        raise ValueError("surface_distances: pred %s and gt %s must be equal-shaped 3-D label volumes" % (pred.shape, gt.shape))
+    if min(pred.shape) < 1 or max(pred.shape) > SD_MAX_DIM:
+        raise ValueError("surface_distances: every dimension must be in [1, %d], got %s" % (SD_MAX_DIM, pred.shape))
+    for name, v in (("pred", pred), ("gt", gt)):
+        if not (np.issubdtype(v.dtype, np.integer) or np.issubdtype(v.dtype, np.bool_)):
+            raise ValueError("surface_distances: %s must hold integer labels, got %s" % (name, v.dtype))
+    sp = (1.0, 1.0, 1.0) if spacing is None else tuple(float(s) for s in np.asarray(spacing, np.float64).reshape(-1))
+    if len(sp) != 3 or not all(math.isfinite(s) and s > 0 for s in sp):
+        raise ValueError("surface_distances: spacing must be 3 positive finite numbers, got %r" % (spacing,))
+    def as_u8(v):
+        if v.dtype == np.uint8:            # uploaded as it is: the kernels count labels >= num_cls as background
+            return np.ascontiguousarray(v)
+        return np.ascontiguousarray(np.where((v >= 0) & (v < num_cls), v, 0), dtype=np.uint8)
+    return as_u8(pred), as_u8(gt), sp
+
+
+def surface_distances(pred, gt, num_cls, spacing=None):
+    """Per-class surface distances of a predicted label volume against a ground truth (medpy.metric.binary.assd / hd, which
+    the papers' evaluation calls without spacing), on the device.
+
+    `pred`, `gt`: host integer arrays [n0, n1, n2] (each n <= 1024); labels outside [0, num_cls) count as background.
+    `spacing`: voxel size along the three axes, default 1 (voxel units).  For each class c >= 1 with A = (pred == c) and
+    B = (gt == c), the border dX is X minus its erosion by the 6-neighbour cross (voxels on the faces of the volume are border
+    voxels) and d(v, S) is the Euclidean distance from v to the nearest voxel of S.  Returns a dict of host arrays [num_cls]:
+      asd_pred_gt  mean of d(v, dB) over v in dA;   asd_gt_pred  mean of d(v, dA) over v in dB;
+      assd         (asd_pred_gt + asd_gt_pred) / 2 (the mean of the two means, like medpy);
+      hd           the larger of the two maxima;
+      border_pred / border_gt  |dA| / |dB| (int64).
+    Index 0 (background) and classes absent from pred or gt are NaN; the border counts say which side was empty.
+    One upload of each volume, one pnp_surface_distance call, one copy back."""
+    p, g, sp = _surface_args(pred, gt, num_cls, spacing)
+    n0, n1, n2 = p.shape
+    nbytes = ctypes.c_longlong(0)
+    call("pnp_surface_distance_workspace", n0, n1, n2, num_cls, ctypes.byref(nbytes))
+    dev = rt.device()
+    dp, dg = torch.from_numpy(p).to(dev), torch.from_numpy(g).to(dev)
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    out = torch.empty((num_cls - 1) * 6, dtype=torch.float64, device=dev)
+    call("pnp_surface_distance", ptr(dp), ptr(dg), n0, n1, n2, num_cls, (ctypes.c_double * 3)(*sp), ptr(ws), nbytes.value,
+         ptr(out), rt.stream())
+    return surface_from_raw(out.cpu().numpy().reshape(num_cls - 1, 6))
+
+
+def surface_from_raw(raw):
+    """surface_distances' per-class dict from pnp_surface_distance's out[C-1][6] table"""
+    raw = np.asarray(raw, np.float64)
+    C = raw.shape[0] + 1
+    res = {k: np.full(C, np.nan) for k in SURFACE_KEYS}
+    res["border_pred"] = np.zeros(C, np.int64)
+    res["border_gt"] = np.zeros(C, np.int64)
+    for c in range(1, C):
+        s_pg, n_p, max_pg, s_gp, n_g, max_gp = raw[c - 1]
+        res["border_pred"][c], res["border_gt"][c] = int(n_p), int(n_g)
+        if n_p > 0 and n_g > 0:
+            res["asd_pred_gt"][c], res["asd_gt_pred"][c] = s_pg / n_p, s_gp / n_g
+            res["assd"][c] = (res["asd_pred_gt"][c] + res["asd_gt_pred"][c]) / 2.0
+            res["hd"][c] = max(max_pg, max_gp)
+    return res
 
 
 def confusion_counts(logits, y):
