@@ -213,7 +213,9 @@ int pnp_crop_concat_fwd(const float* x1, const float* x2, float* out, int B, int
                         void* stream);
 int pnp_crop_concat_bwd(const float* dout, float* dx1, float* dx2, int B, int H1, int W1, int C1, int H2, int W2, int C2,
                         void* stream);
-/* tf.pad(..., 'SYMMETRIC') by p on each spatial side (layers.py:19-23,68-72) */
+/* tf.pad(..., 'SYMMETRIC') by p on each spatial side (layers.py:19-23,68-72) and its adjoint (MirrorPadGrad: each dx element
+ * sums the up to 3 x 3 padded positions that mirror onto it).  Both directions require 0 <= p <= H, W (PNP_ERR_UNSUPPORTED
+ * otherwise), as TensorFlow's SYMMETRIC mode does. */
 int pnp_mirror_pad_fwd(const float* x, float* y, int B, int H, int W, int C, int p, void* stream);
 int pnp_mirror_pad_bwd(const float* dy, float* dx, int B, int H, int W, int C, int p, void* stream);
 /* PS / _phase_shift (ops.py:3-27): X[B,a,b,G*r*r] -> out[B,a*r,b*r, Ctot] channels [coff, coff+ntile*G),

@@ -1362,7 +1362,7 @@ extern "C" int pnp_mirror_pad_fwd(const float* x, float* y, int B, int H, int W,
 
 extern "C" int pnp_mirror_pad_bwd(const float* dy, float* dx, int B, int H, int W, int C, int p, void* stream) {
   if (!dy || !dx || B <= 0 || H <= 0 || W <= 0 || C <= 0 || p < 0) return PNP_ERR_BAD_ARG;
-  if (2 * p > H || 2 * p > W) return PNP_ERR_UNSUPPORTED;
+  if (p > H || p > W) return PNP_ERR_UNSUPPORTED;
   long long total = (long long)B * H * W * C;
   pnp_launch(mirror_pad_bwd_kernel, grid_for(total, 256 * 8), 256, 0, S_, dy, dx, B, H, W, C, p);
   PNP_LAUNCH_CHECK();
@@ -1604,4 +1604,4 @@ extern "C" const char* pnp_error_string(int code) {
   }
 }
 
-extern "C" int pnp_version(void) { return 101; }
+extern "C" int pnp_version(void) { return 102; }

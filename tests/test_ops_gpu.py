@@ -47,6 +47,7 @@ CONV_CASES = [
     (2, 16, 16, 16, 32, 5, 4, 1, "SAME"),      # m_cls_2_3: 5x5 stride 4
     (2, 4, 4, 64, 64, 3, 2, 1, "SYMMETRIC"),   # cls_6
     (2, 8, 8, 32, 64, 5, 4, 1, "SYMMETRIC"),   # m_cls_4
+    (2, 3, 3, 8, 8, 5, 1, 1, "SYMMETRIC"),     # 5x5 mirror pad by 2 on a 3x3 map: a border row mirrors onto 3 padded rows
     (2, 16, 16, 5, 16, 3, 2, 1, "SAME"),       # mask_cls_1: Cin=5
     (3, 12, 20, 24, 40, 3, 1, 1, "SAME"),      # odd sizes / ragged tiles
     (1, 7, 9, 8, 12, 3, 2, 1, "SAME"),         # odd spatial, stride 2
