@@ -24,7 +24,7 @@ def main():
     ap.add_argument("--settle", type=int, default=30)
     ap.add_argument("--check", type=int, default=4)
     a = ap.parse_args()
-    from tests.test_parity_configs_gpu import seg_pair
+    from tests.models import seg_pair
     from pnp_b200 import runtime as rt
     from pnp_b200.data import SyntheticSource
     from oracle.pnp_graphs import OracleSegmenter

@@ -31,7 +31,7 @@ def sample_positions(B, seed=20260924):
 
 def main():
     from tests import test_reference_graph_in_opencv_cpu as G
-    from tests.test_parity_configs_gpu import _bn_noise
+    from tests.models import bn_noise as _bn_noise
     from oracle.pnp_graphs import OracleSegmenter, OracleAdversarial, init_numpy_params, synthetic_images
     REF = json.load(open(os.path.join(HERE, "reference_graph_trace.json")))
     B = G.B

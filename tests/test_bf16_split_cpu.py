@@ -6,7 +6,8 @@ import pytest
 import torch
 
 from oracle import bf16_split as S
-from tests.test_tc_split_exact_gpu import CASES, edge_values, expected_ksplit, geom_of, operands
+from tests.cabi import expected_ksplit
+from tests.test_tc_split_exact_gpu import CASES, edge_values, geom_of, operands
 
 U32 = 2.0 ** -23
 

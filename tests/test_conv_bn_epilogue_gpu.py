@@ -19,12 +19,9 @@ import subprocess
 import pytest
 import torch
 
-from oracle import philox
+from tests.cabi import DEV, ROOT, block_n, crosses_ntile, drop_cfg, drop_mask, last_config, lib, sm_count, split_dev, split_w_dev
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "medical-cross-modality-domain-adaptation_b200", "libpnp_b200.so")
-DEV = "cuda"
-SEED, DROP_STREAM = 0x1234_5678_9ABC, 11
 
 # (id, B, H, W, Cin, Cout): 3x3 SAME stride-1 convolutions.  Widths 40 and 56 leave 8 / 16 of each 128-row tile past the image
 # row, and 40 / 56 rows are not a multiple of the tile's 3 / 2 rows: the last row of tiles is ragged too.
@@ -37,68 +34,23 @@ CASES = [
 CASE_IDS = [c[0] for c in CASES]
 
 
-def _lib():
-    import pnp_b200  # noqa: F401
-    from pnp_b200 import _C, runtime as rt
-    if not rt.tc_available():
-        pytest.fail("wgmma path unavailable on this device -- it must be the one that runs on H100")
-    return _C, rt
-
-
 def _geom(_C, case):
     _, B, H, W, Cin, Cout = case
     return _C.ConvGeom(B, H, W, Cin, H, W, Cout, 3, 3, 1, 1, 1, 1)
 
 
-def _block_n(cout):
-    return 128 if cout % 128 == 0 else (64 if cout % 64 == 0 else (32 if cout % 32 == 0 else 16))
-
-
-def _tiles(g):
-    """(m-tiles, n-tiles) of the forward launcher (conv_tc.cu choose_tile / run_tc, stride 1)"""
-    tw, th = (128, 1) if g.Wo >= 128 else (g.Wo, min(128 // g.Wo, g.Ho))
-    tn = min(max(128 // (tw * th), 1), g.B) if th == g.Ho else 1
-    return (-(-g.Wo // tw)) * (-(-g.Ho // th)) * (-(-g.B // tn)), g.Cout // _block_n(g.Cout)
-
-
-def _crosses_ntile(g, sms):
-    """does some persistent CTA walk tiles of two different n-tiles (tile t -> n-tile t % n_tiles, CTA b walks b, b + sms, ..)"""
-    mt, nt = _tiles(g)
-    total = mt * nt
-    return any(len({t % nt for t in range(b, total, sms)}) > 1 for b in range(min(sms, total)))
-
-
-def _planes(_C, rt, x, nterms):
-    hi = torch.empty(x.shape, dtype=torch.bfloat16, device=DEV)
-    lo = torch.empty(x.shape, dtype=torch.bfloat16, device=DEV) if nterms == 3 else None
-    _C.call("pnp_split_bf16", _C.ptr(x), _C.ptr(hi), _C.ptr(lo), x.numel(), rt.stream())
-    return hi, lo
-
-
-def _wplanes(_C, rt, w, nterms):
-    kh, kw, cin, cout = w.shape
-    hi = torch.empty(w.numel(), dtype=torch.bfloat16, device=DEV)
-    lo = torch.empty_like(hi) if nterms == 3 else None
-    _C.call("pnp_split_weight_bf16", _C.ptr(w), _C.ptr(hi), _C.ptr(lo), kh, kw, cin, cout, 0, 0, rt.stream())
-    return hi, lo
-
-
 def _fwd_bn(_C, rt, g, x, w, nterms, keep=None):
     """-> (y, sum, sumsq) of one pnp_conv2d_tc_fwd launch with fused BN sums"""
-    xh, xl = _planes(_C, rt, x, nterms)
-    wh, wl = _wplanes(_C, rt, w, nterms)
+    xh, xl = split_dev(_C, rt, x, nterms)
+    wh, wl = split_w_dev(_C, rt, w, False, nterms)
     y = torch.full((g.B, g.Ho, g.Wo, g.Cout), float("nan"), device=DEV)
     s = torch.zeros(2, g.Cout, dtype=torch.float64, device=DEV)
-    drop = None
-    if keep is not None:
-        seed = torch.tensor([SEED], dtype=torch.int64, device=DEV)
-        drop = _C.DropCfg(seed.data_ptr(), DROP_STREAM, keep)
+    drop, seed_t = drop_cfg(_C, keep) if keep is not None else (None, None)
     _C.call("pnp_conv2d_tc_fwd", _C.ptr(xh), _C.ptr(xl), _C.ptr(wh), _C.ptr(wl), _C.ptr(y), ctypes.byref(g), nterms,
             None if drop is None else ctypes.byref(drop), 0, _C.ptr(s[0]), _C.ptr(s[1]), rt.stream())
     torch.cuda.synchronize()
-    n_, k_, ks = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_int(0)
-    _C.lib.pnp_tc_last_config(ctypes.byref(n_), ctypes.byref(k_), ctypes.byref(ks))
-    assert n_.value == _block_n(g.Cout) and ks.value == 1, "expected the fused-epilogue path, got %s" % ((n_.value, k_.value, ks.value),)
+    n, _, ks = last_config(_C)
+    assert n == block_n(g.Cout) and ks == 1, "expected the fused-epilogue path, got %s" % (last_config(_C),)
     return y, s[0], s[1]
 
 
@@ -107,10 +59,10 @@ def _fwd_bn(_C, rt, g, x, w, nterms, keep=None):
 @pytest.mark.parametrize("nterms", [3, 1])
 @pytest.mark.parametrize("case", CASES, ids=CASE_IDS)
 def test_bn_sums_match_fp64(case, nterms, keep):
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     g = _geom(_C, case)
-    if case[-1] // _block_n(case[-1]) > 1:
-        assert _crosses_ntile(g, torch.cuda.get_device_properties(0).multi_processor_count), "no CTA flushes mid-list"
+    if case[-1] // block_n(case[-1]) > 1:
+        assert crosses_ntile(g, sm_count()), "no CTA flushes mid-list"
     gen = torch.Generator().manual_seed(case[-1] + nterms)
     x = (torch.randn(g.B, g.H, g.W, g.Cin, generator=gen) + 0.3).to(DEV)
     w = (torch.randn(3, 3, g.Cin, g.Cout, generator=gen) * 0.05).to(DEV)
@@ -130,7 +82,7 @@ def test_bn_sums_match_fp64(case, nterms, keep):
 def test_bn_sums_exact_on_integers(case, nterms):
     """x, w in {-1, 0, 1} (exact in the hi plane): |z| <= 9 Cin, so a warp's 16-row fp32 sum of z^2 stays below 2^24 and is exact
     for Cin <= 64 (and for Cin <= 32 with keep = 0.5, whose multiplier is 2); every fp64 sum after it is exact as well"""
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     g = _geom(_C, case)
     gen = torch.Generator().manual_seed(3 * case[-1] + nterms)
     x = torch.randint(-1, 2, (g.B, g.H, g.W, g.Cin), generator=gen).float().to(DEV)
@@ -141,8 +93,7 @@ def test_bn_sums_exact_on_integers(case, nterms):
         y, s1, s2 = _fwd_bn(_C, rt, g, x, w, nterms, keep)
         want = ref
         if keep is not None:
-            mask = philox.dropout_mult(SEED, DROP_STREAM, keep, ref.numel())
-            want = ref * torch.from_numpy(mask).reshape(ref.shape).to(DEV).double()
+            want = ref * drop_mask(drop_cfg(_C, keep)[0], ref.shape).double()
         assert torch.equal(y.double(), want), "%s nterms %d keep %s: output not exact" % (case[0], nterms, keep)
         z = want.reshape(-1, g.Cout)
         assert torch.equal(s1, z.sum(0)), "%s nterms %d keep %s: BN sum not exact" % (case[0], nterms, keep)

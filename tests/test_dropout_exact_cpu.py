@@ -11,7 +11,7 @@ import pytest
 from oracle import bf16_split as S
 from oracle import philox as PH
 from tests.test_dropout_exact_gpu import GRID_CAP_N, KEEPS, SEEDS, SIMT_CASES, STREAMS, TC_CASES
-from tests.test_tc_split_exact_gpu import expected_ksplit
+from tests.cabi import expected_ksplit
 
 KAT = [  # Random123 kat_vectors, philox4x32 10 rounds: (ctr, key, output)
     ((0, 0, 0, 0), (0, 0), (0x6627E8D5, 0xE169C58D, 0xBC57AC4C, 0x9B00DBD8)),

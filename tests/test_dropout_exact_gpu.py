@@ -6,13 +6,10 @@ a. pnp_dropout_apply: y == fl32(x * mult) over seeds {0, 0x5EED, 2^63 - 1, 2^64 
 b. the SIMT forward convolution (float4 and scalar stores, with accumulate) and the wgmma forward convolution (plain and fused
    epilogue, nterms 1 and 3, every accumulator width 16 / 32 / 64 / 128, a ragged last tile, a split-K layer) on integer
    operands: y == [y0 +] fl32(mult * conv) with conv the exact fp64 convolution.  (The batch-norm backward entry points are
-   pinned to the same reference through drop_mask of tests/test_tc_split_exact_gpu.py, which now draws from it.)
+   pinned to the same reference through drop_mask of tests/cabi.py, which now draws from it.)
 c. pnp_seed_advance against the Python LCG, runtime.manual_seed, a captured graph of [pnp_seed_advance, pnp_dropout_apply];
 d. the seed-advance -> dropout and seed-advance -> convolution sequences again under PNP_PDL=1, in their own process."""
 import ctypes
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -20,11 +17,9 @@ import torch
 import torch.nn.functional as F
 
 from oracle import philox as PH
-from tests.test_tc_split_exact_gpu import last_config, split_dev, split_w_dev
+from tests.cabi import DEV, last_config, lib, rerun, split_dev, split_w_dev
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEV = "cuda"
 
 SEEDS = [0, 0x5EED, (1 << 63) - 1, (1 << 64) - 1]
 STREAMS = [0, 1, (1 << 32) - 1, (1 << 32) + 5, (1 << 64) - 1]
@@ -42,12 +37,6 @@ TC_CASES = [
     ("n128_8imgs_per_tile", 537, 4, 4, 128, 128, 0.75, 128, False),   # 8 images per tile, the last tile holds one
     ("splitk", 1, 8, 8, 512, 64, 0.5, 64, True),                # 1 tile, 72 k-blocks: split along K; mult 2 keeps it exact
 ]
-
-
-def _lib():
-    import pnp_b200  # noqa: F401
-    from pnp_b200 import _C, runtime as rt
-    return _C, rt
 
 
 def seed_tensor(s):
@@ -81,7 +70,7 @@ def assert_same(tag, got, want):
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("keep", KEEPS)
 def test_dropout_apply_matches_philox(keep):
-    _C, rt = _lib()
+    _C, rt = lib()
     gen = torch.Generator(device=DEV).manual_seed(7)
     n = 4099
     x = torch.randn(n, generator=gen, device=DEV)
@@ -95,7 +84,7 @@ def test_dropout_apply_matches_philox(keep):
 
 def test_dropout_apply_tails():
     """n = 1 .. 9: every value of n & 3, the scalar tail alone and after whole quads"""
-    _C, rt = _lib()
+    _C, rt = lib()
     seed_t = seed_tensor(SEEDS[3])
     for n in range(1, 10):
         x = torch.randn(n, device=DEV)
@@ -106,7 +95,7 @@ def test_dropout_apply_tails():
 
 def test_dropout_apply_grid_stride_and_in_place():
     """n above 4 * 8448 * 1024 (grid-stride loop past the CTA cap) with a tail, in place"""
-    _C, rt = _lib()
+    _C, rt = lib()
     x = torch.randn(GRID_CAP_N, generator=torch.Generator(device=DEV).manual_seed(3), device=DEV)
     want = x * ref_mult(SEEDS[2], STREAMS[4], 0.3, (GRID_CAP_N,))
     seed_t = seed_tensor(SEEDS[2])
@@ -115,7 +104,7 @@ def test_dropout_apply_grid_stride_and_in_place():
 
 
 def test_dropout_disabled_paths():
-    _C, rt = _lib()
+    _C, rt = lib()
     x = torch.randn(1001, device=DEV)
     seed_t = seed_tensor(5)
     for tag, cfg in (("NULL seed", cfg_for(_C, None, 3, 0.5)), ("keep 1", cfg_for(_C, seed_t, 3, 1.0)), ("no cfg", None)):
@@ -151,7 +140,7 @@ def conv_exact(x, w):
 
 @pytest.mark.parametrize("case", SIMT_CASES, ids=[c[0] for c in SIMT_CASES])
 def test_simt_conv_dropout(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, B, H, W, Cin, Cout, keep = case
     x, w = _int_operands(B, H, W, Cin, Cout, 31)
     ref = conv_exact(x, w)
@@ -172,9 +161,7 @@ def test_simt_conv_dropout(case):
 @pytest.mark.parametrize("nterms", [1, 3])
 @pytest.mark.parametrize("case", TC_CASES, ids=[c[0] for c in TC_CASES])
 def test_tc_conv_dropout(case, nterms):
-    _C, rt = _lib()
-    if not rt.tc_available():
-        pytest.fail("wgmma path unavailable on this device")
+    _C, rt = lib(require_tc=True)
     tag, B, H, W, Cin, Cout, keep, block_n, split = case
     x, w = _int_operands(B, H, W, Cin, Cout, 37)
     ref = conv_exact(x, w)
@@ -214,7 +201,7 @@ def test_tc_conv_dropout(case, nterms):
 # c. seed advance, manual_seed, graphs
 # ------------------------------------------------------------------------------------------------
 def test_seed_advance_matches_lcg():
-    _C, rt = _lib()
+    _C, rt = lib()
     for s in SEEDS + [0x1234_5678_9ABC]:
         t = seed_tensor(s)
         for k in range(1, 6):
@@ -224,7 +211,7 @@ def test_seed_advance_matches_lcg():
 
 
 def test_manual_seed_masks_the_sign_bit():
-    _, rt = _lib()
+    _, rt = lib()
     for s in (0, 5, (1 << 63) - 1, 1 << 63, (1 << 64) - 1, 0xDEAD_BEEF_0123_4567_89):
         rt.manual_seed(s)
         assert int(rt.rng.seed_t.item()) == s & ((1 << 63) - 1)
@@ -233,7 +220,7 @@ def test_manual_seed_masks_the_sign_bit():
 
 def test_seed_advance_then_producers():
     """the advance and the draw back to back in stream order: the draw must see the advanced seed"""
-    _C, rt = _lib()
+    _C, rt = lib()
     seed = SEEDS[1]
     x, w = _int_operands(2, 16, 16, 16, 16, 41)
     ref = conv_exact(x, w)
@@ -263,7 +250,7 @@ def test_seed_advance_then_producers():
 
 def test_graph_replays_draw_fresh_masks():
     """[pnp_seed_advance, pnp_dropout_apply] captured once, replayed 3 times: replay k draws the mask of LCG^k(seed)"""
-    _C, rt = _lib()
+    _C, rt = lib()
     seed = SEEDS[3]
     seed_t = seed_tensor(seed)
     x = torch.randn(10007, device=DEV)
@@ -287,11 +274,10 @@ def test_graph_replays_draw_fresh_masks():
 # ------------------------------------------------------------------------------------------------
 # d. PDL
 # ------------------------------------------------------------------------------------------------
+PDL_TESTS = ("seed_advance_matches_lcg", "seed_advance_then_producers", "graph_replays_draw_fresh_masks", "dropout_apply_tails")
+
+
 @pytest.mark.timeout(300)
 def test_exact_cases_under_pdl():
-    env = dict(os.environ, PNP_PDL="1")
-    code = ("import sys; sys.path.insert(0, %r); from tests import test_dropout_exact_gpu as T; "
-            "T.test_seed_advance_matches_lcg(); T.test_seed_advance_then_producers(); T.test_graph_replays_draw_fresh_masks(); "
-            "T.test_dropout_apply_tails(); print('pdl ok')" % ROOT)
-    r = subprocess.run([sys.executable, "-c", code], env=env, cwd=ROOT, capture_output=True, text=True, timeout=280)
-    assert r.returncode == 0 and "pdl ok" in r.stdout, r.stdout[-2000:] + r.stderr[-4000:]
+    passed, _ = rerun({"PNP_PDL": "1"}, __file__, " or ".join(PDL_TESTS))
+    assert passed == len(PDL_TESTS), passed

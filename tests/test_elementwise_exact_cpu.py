@@ -6,14 +6,11 @@ import torch
 
 from oracle import elementwise_exact as E
 from oracle import tf14_torch as T
+from tests.cabi import ints, pick
 from tests.test_elementwise_exact_gpu import (APPLY_SHAPES, BIG, BWD_SHAPES, REDUCE_CASES, SEG_P, VAR_CASES,
                                               invstd_sweep_variances, var_for_invstd)
 
 REGIMES = {"tpr%d" % (1 << i) for i in range(9)} | {"idle_lanes", "ragged", "odd_rows", "m_lt_rstep", "capped", "promoted"}
-
-
-def _ints(shape, lo, hi, gen, scale=1.0):
-    return torch.randint(lo, hi + 1, shape, generator=gen).double() * scale
 
 
 # ------------------------------------------------------------------------------------------------
@@ -204,7 +201,7 @@ def test_exact_stats_reject_a_row_at_a_cta_boundary(mode):
     """a row left out of (or counted twice in) the BN sums at a CTA boundary changes an exact integer sum"""
     for tag, M, C in _small_reduce_cases():
         gen = torch.Generator().manual_seed(M + C)
-        z = _ints((M, C), -8, 8, gen)
+        z = ints((M, C), -8, 8, gen).double()
         r = _boundary_row(M, C)
         s1, s2, _ = E.bn_stats_ref(z)
         row = z[r]
@@ -212,7 +209,7 @@ def test_exact_stats_reject_a_row_at_a_cta_boundary(mode):
         assert not (torch.equal(s1 + sign * row, s1) and torch.equal(s2 + sign * row * row, s2)), tag
         # the same row in the g-sums of the backward reduce
         gen = torch.Generator().manual_seed(7 + M + C)
-        dy = _ints((M, C), -8, 8, gen, 5.0)
+        dy = ints((M, C), -8, 8, gen, 5.0).double()
         g, sg, _, _, _ = E.bn_bwd_reduce_ref(dy, dy, z, torch.zeros(C), torch.ones(C), E.NONE)
         assert not torch.equal(sg + sign * g[r].double(), sg), tag
 
@@ -256,8 +253,8 @@ def test_tau_finalize_rejects_the_biased_moving_variance():
 def test_exact_reduce_rejects_slope_one_at_zero(act):
     for tag, M, C in _small_reduce_cases():
         gen = torch.Generator().manual_seed(M + C)
-        z, mean = _ints((M, C), -8, 8, gen), _ints((C,), -2, 2, gen)
-        dy, y = _ints((M, C), -8, 8, gen, 5.0), _ints((M, C), -3, 3, gen)
+        z, mean = ints((M, C), -8, 8, gen).double(), ints((C,), -2, 2, gen).double()
+        dy, y = ints((M, C), -8, 8, gen, 5.0).double(), ints((M, C), -3, 3, gen).double()
         if not bool(((y == 0) & (dy != 0)).any()):
             continue                                           # M = 1: the row may hold no zero y
         good = E.bn_bwd_reduce_ref(dy, y, z, mean, torch.ones(C), act)
@@ -267,12 +264,12 @@ def test_exact_reduce_rejects_slope_one_at_zero(act):
 
 def _bwd_operands_cpu(M, C, seed, keep=None):
     gen = torch.Generator().manual_seed(seed)
-    z, mean = _ints((M, C), -8, 8, gen), _ints((C,), -2, 2, gen)
-    invstd = torch.tensor([1.0, 0.5])[torch.randint(0, 2, (C,), generator=gen)].double()
+    z, mean = ints((M, C), -8, 8, gen).double(), ints((C,), -2, 2, gen).double()
+    invstd = pick((C,), [1.0, 0.5], gen).double()
     invstd[0] = 0.5
-    dy = _ints((M, C), -8, 8, gen, 5.0)
-    gamma = torch.tensor([0.5, 1.0, 1.5, 2.0])[torch.randint(0, 4, (C,), generator=gen)].double()
-    c1, c2 = _ints((C,), -8, 8, gen, 0.25), _ints((C,), -8, 8, gen, 0.25)
+    dy = ints((M, C), -8, 8, gen, 5.0).double()
+    gamma = pick((C,), [0.5, 1.0, 1.5, 2.0], gen).double()
+    c1, c2 = ints((C,), -8, 8, gen, 0.25).double(), ints((C,), -8, 8, gen, 0.25).double()
     c2[0] = 1.0
     mask = None if keep is None else (torch.rand(M, C, generator=gen) < keep).float() / keep
     return z, mean, invstd, dy, gamma, c1, c2, mask

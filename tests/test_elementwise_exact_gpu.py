@@ -13,22 +13,16 @@ e. the exact reduce and apply cases again under PNP_PDL=1, in their own process.
 
 Each real-valued test prints its worst ratio |got - ref| / magnitude next to TAU."""
 import ctypes
-import os
-import subprocess
-import sys
-import time
 
 import pytest
 import torch
 
 from oracle import bf16_split as S
 from oracle import elementwise_exact as E
-from tests.test_tc_split_exact_gpu import _assert_planes, _planes, drop_cfg, drop_mask
+from tests.cabi import (BAD_ARG, DEV, UNSUPPORTED, assert_planes, assert_untouched, dev_gen, drop_cfg, drop_mask, empty_planes, ints,
+                        lib, pick, ptr, rerun, snapshot, sync)
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEV = "cuda"
-BAD_ARG, UNSUPPORTED = 100001, 100002
 
 # (id, M, C) of the BN reductions; the CPU file checks that together they reach every regime of E.reduce_regimes
 REDUCE_CASES = [
@@ -45,30 +39,6 @@ APPLY_SHAPES = [("C4", 1001, 4), ("C1024", 37, 1024), ("C96", 1000, 96), ("grid_
 SKIPS = {4: [(4, 0)], 1024: [(512, 256), (4, 1020)], 96: [(32, 40), (96, 0)], 16: [(8, 8)]}
 BWD_SHAPES = [("C64", 3000, 64), ("C1024", 4, 1024), ("C4_M1", 1, 4), ("grid_stride_C16", 600000, 16)]
 SEG_P = [524288, 100003]
-
-
-def _lib():
-    import pnp_b200  # noqa: F401
-    from pnp_b200 import _C, runtime as rt
-    return _C, rt
-
-
-def ptr(t):
-    return None if t is None else t.data_ptr()
-
-
-def _gen(seed):
-    return torch.Generator(device=DEV).manual_seed(seed)
-
-
-def ints(shape, lo, hi, gen, scale=1.0):
-    """uniform integers in [lo, hi] as fp32, times scale"""
-    return torch.randint(lo, hi + 1, shape, generator=gen, device=DEV).float() * scale
-
-
-def pick(shape, values, gen):
-    v = torch.tensor(values, dtype=torch.float32, device=DEV)
-    return v[torch.randint(0, len(values), shape, generator=gen, device=DEV)]
 
 
 def var_for_invstd(inv):
@@ -96,16 +66,12 @@ def check(key, tag, got, ref, mag):
     assert bad == 0, "%s %s: %d elements beyond tau %.3e (worst ratio %.3e)" % (key, tag, bad, tau, ratio)
 
 
-def sync():
-    torch.cuda.synchronize()
-
-
 # ------------------------------------------------------------------------------------------------
 # a. BN reductions, exact
 # ------------------------------------------------------------------------------------------------
 def reduce_operands(M, C, seed):
     """integer z in [-8, 8], integer mean, invstd in {1, .5}, dy in 5 * [-8, 8] (fl(0.2f * dy) = dy / 5), y in [-3, 3]"""
-    gen = _gen(seed)
+    gen = dev_gen(seed)
     z = ints((M, C), -8, 8, gen)
     mean = ints((C,), -2, 2, gen)
     invstd = pick((C,), [1.0, 0.5], gen)
@@ -121,9 +87,9 @@ def reduce_precondition(term_max):
 
 @pytest.mark.parametrize("case", REDUCE_CASES, ids=[c[0] for c in REDUCE_CASES])
 def test_bn_stats_exact(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, M, C = case
-    gen = _gen(M + C)
+    gen = dev_gen(M + C)
     z = ints((M, C), -8, 8, gen)
     reduce_precondition(64)
     init = ints((C,), -3, 3, gen).double()
@@ -140,12 +106,12 @@ def test_bn_stats_exact(case):
 def test_bn_bwd_reduce_exact(case):
     """pnp_bn_bwd_reduce (g and sums, sign from y) and pnp_bn_bwd_reduce_sums (sign from y and from y_hi) against fp64 sums of
     the same g: all three sums are equal, so the sums-only route is the sums of the g-writing route"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, M, C = case
     z, mean, invstd, dy, y = reduce_operands(M, C, 7 + M + C)
     yhi = y.to(torch.bfloat16)
     reduce_precondition(40 * 10)
-    gen = _gen(3)
+    gen = dev_gen(3)
     for act in ((E.LRELU,) if tag in BIG else (E.NONE, E.RELU, E.LRELU)):
         g_ref, sg_ref, sgx_ref, _, _ = E.bn_bwd_reduce_ref(dy, y, z, mean, invstd, act)
         init = ints((C,), -3, 3, gen).double()
@@ -175,9 +141,9 @@ def _skip_variants(C):
 @pytest.mark.parametrize("shape", APPLY_SHAPES, ids=[s[0] for s in APPLY_SHAPES])
 def test_bn_act_apply_exact(shape):
     """dyadic scale / shift and integer z, skip: fma + skip + act is exact; y only, and y with planes (planes == split(y))"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, M, C = shape
-    gen = _gen(M * 3 + C)
+    gen = dev_gen(M * 3 + C)
     z = ints((M, C), -8, 8, gen)
     scale = pick((C,), [-1.5, -1.0, -0.5, 0.5, 1.0, 2.0], gen)
     shift = ints((C,), -4, 4, gen, 0.5)
@@ -187,14 +153,14 @@ def test_bn_act_apply_exact(shape):
             y_ref, _ = E.bn_apply_ref(z, scale, shift, skip, off, act)
             for planes in (False, True):
                 y = torch.full((M, C), float("nan"), device=DEV)
-                hi, lo = _planes((M, C), 3) if planes else (None, None)
+                hi, lo = empty_planes((M, C), 3) if planes else (None, None)
                 _C.call("pnp_bn_act_apply", ptr(z), ptr(scale), ptr(shift), ptr(skip), Cs or 0, off, act, ptr(y), ptr(hi), ptr(lo),
                         M, C, rt.stream())
                 sync()
                 what = "%s skip=%s@%d act %d planes %d" % (tag, Cs, off, act, planes)
                 assert torch.equal(y, y_ref), what
                 if planes:
-                    _assert_planes(what, hi, lo, y_ref)
+                    assert_planes(what, hi, lo, y_ref)
 
 
 @pytest.mark.parametrize("training", [0, 1])
@@ -203,9 +169,9 @@ def test_bn_apply_fused_exact(shape, training):
     """pnp_bn_apply_fused with statistics that make invstd exactly 1 or 2 (training 0: moving statistics; training 1: fp64
     sums that are M times an integer mean and an exact variance): scale, shift and y are exact; mean_out / invstd_out are the
     statistics; y only, planes only and both write the same values; training 1 updates the moving statistics (within TAU)"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, M, C = shape
-    gen = _gen(M + 5 * C + training)
+    gen = dev_gen(M + 5 * C + training)
     z = ints((M, C), -8, 8, gen)
     inv = pick((C,), [1.0, 2.0], gen)
     var = torch.where(inv == 1.0, torch.full_like(inv, var_for_invstd(1.0)), torch.full_like(inv, var_for_invstd(2.0)))
@@ -231,7 +197,7 @@ def test_bn_apply_fused_exact(shape, training):
             got = {}
             for mode in ("y", "planes", "both"):
                 y = torch.full((M, C), float("nan"), device=DEV) if mode != "planes" else None
-                hi, lo = _planes((M, C), 3) if mode != "y" else (None, None)
+                hi, lo = empty_planes((M, C), 3) if mode != "y" else (None, None)
                 mm, mv = mm_in.clone(), mv_in.clone()
                 mo, io = torch.full((C,), float("nan"), device=DEV), torch.full((C,), float("nan"), device=DEV)
                 _C.call("pnp_bn_apply_fused", ptr(z), ptr(s1), ptr(s2), M, C, ptr(gamma), ptr(beta), ptr(mm), ptr(mv), training,
@@ -243,7 +209,7 @@ def test_bn_apply_fused_exact(shape, training):
                 if y is not None:
                     assert torch.equal(y, y_ref), what
                 if hi is not None:
-                    _assert_planes(what, hi, lo, y_ref)
+                    assert_planes(what, hi, lo, y_ref)
                     got[mode] = (S.bits(hi), S.bits(lo))
                 if not training:
                     assert torch.equal(mm, mm_in) and torch.equal(mv, mv_in), what + ": moving statistics changed"
@@ -261,7 +227,7 @@ def test_bn_apply_fused_exact(shape, training):
 # a. BN backward apply, exact
 # ------------------------------------------------------------------------------------------------
 def bwd_operands(M, C, seed):
-    gen = _gen(seed)
+    gen = dev_gen(seed)
     z, mean, invstd, dy, y = reduce_operands(M, C, seed + 1)
     gamma = pick((C,), [0.5, 1.0, 1.5, 2.0], gen)
     c1 = ints((C,), -8, 8, gen, 0.25)
@@ -277,13 +243,13 @@ def bwd_operands(M, C, seed):
 def test_bn_bwd_apply_exact(shape, training, keep):
     """_bwd_finalize -> _bwd_apply, _bwd_apply_fused and _bwd_apply_direct (every act, sign from y and from y_hi, dz and
     planes-only) against the fp64 dz, the dropout multiplier applied as the final fp32 multiply; dgamma / dbeta accumulate"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, M, C = shape
     z, mean, invstd, dy, y, gamma, c1, c2, sg, sgx, dg0, db0 = bwd_operands(M, C, 11 * M + C + training)
     yhi = y.to(torch.bfloat16)
     dcfg, _seed = drop_cfg(_C, keep) if keep < 1 else (None, None)
     dref = None if dcfg is None else ctypes.byref(dcfg)
-    mask = drop_mask(_C, rt, dcfg, (M, C)) if dcfg is not None else None
+    mask = drop_mask(dcfg, (M, C)) if dcfg is not None else None
     # finalize: coef exact, dgamma / dbeta += sums
     coef = torch.full((2 * C,), float("nan"), device=DEV)
     dg, db = dg0.clone(), db0.clone()
@@ -294,13 +260,13 @@ def test_bn_bwd_apply_exact(shape, training, keep):
     # separate apply from g = dy
     dz_ref, _ = E.bn_bwd_apply_ref(dy, z, mean, invstd, gamma, c1, c2, training, mask)
     dz = torch.full((M, C), float("nan"), device=DEV)
-    hi, lo = _planes((M, C), 3)
+    hi, lo = empty_planes((M, C), 3)
     _C.call("pnp_bn_bwd_apply", ptr(dy), ptr(z), ptr(mean), ptr(invstd), ptr(gamma), ptr(coef), training, dref, ptr(dz), ptr(hi),
             ptr(lo), M, C, rt.stream())
     sync()
     what = "%s train %d keep %g" % (tag, training, keep)
     assert torch.equal(dz, dz_ref), what + ": pnp_bn_bwd_apply"
-    _assert_planes(what, hi, lo, dz_ref)
+    assert_planes(what, hi, lo, dz_ref)
     # fused: the same dz, dgamma / dbeta accumulated by CTA 0
     dz = torch.full((M, C), float("nan"), device=DEV)
     dg, db = dg0.clone(), db0.clone()
@@ -308,7 +274,7 @@ def test_bn_bwd_apply_exact(shape, training, keep):
             ptr(dg), ptr(db), ptr(dz), ptr(hi), ptr(lo), rt.stream())
     sync()
     assert torch.equal(dz, dz_ref), what + ": pnp_bn_bwd_apply_fused"
-    _assert_planes(what + " fused", hi, lo, dz_ref)
+    assert_planes(what + " fused", hi, lo, dz_ref)
     assert torch.equal(dg, dg0 + sgx.float()) and torch.equal(db, db0 + sg.float()), what + ": fused dgamma / dbeta"
     # direct: g = dy * act'(y) recomputed, sign from y or y_hi; dz = NULL writes the same planes
     for act in (E.NONE, E.RELU, E.LRELU):
@@ -318,7 +284,7 @@ def test_bn_bwd_apply_exact(shape, training, keep):
             planes = []
             for with_dz in (True, False):
                 dz = torch.full((M, C), float("nan"), device=DEV) if with_dz else None
-                hi, lo = _planes((M, C), 3)
+                hi, lo = empty_planes((M, C), 3)
                 dg, db = dg0.clone(), db0.clone()
                 _C.call("pnp_bn_bwd_apply_direct", ptr(dy), ptr(y) if src == "y" else None, ptr(yhi) if src == "y_hi" else None, act,
                         ptr(z), ptr(mean), ptr(invstd), ptr(gamma), ptr(sg), ptr(sgx), M, C, training, dref, ptr(dg), ptr(db), ptr(dz),
@@ -327,7 +293,7 @@ def test_bn_bwd_apply_exact(shape, training, keep):
                 w = "%s direct act %d %s dz %d" % (what, act, src, with_dz)
                 if with_dz:
                     assert torch.equal(dz, dref_act), w
-                _assert_planes(w, hi, lo, dref_act)
+                assert_planes(w, hi, lo, dref_act)
                 assert torch.equal(dg, dg0 + sgx.float()), w + ": dgamma"
                 planes.append((S.bits(hi), S.bits(lo)))
             assert torch.equal(planes[0][0], planes[1][0]) and torch.equal(planes[0][1], planes[1][1]), w
@@ -336,7 +302,7 @@ def test_bn_bwd_apply_exact(shape, training, keep):
 def test_bn_bwd_routes_are_bit_equal():
     """randn operands, training with dropout: _bwd_apply_fused == _bwd_reduce -> _bwd_finalize -> _bwd_apply, and
     _bwd_apply_direct(dy, y) == pnp_act_bwd -> _bwd_apply_fused, bit for bit (the same sums feed both routes)"""
-    _C, rt = _lib()
+    _C, rt = lib()
     M, C = 3000, 64
     g0 = torch.Generator().manual_seed(5)
     f = lambda *s: torch.randn(*s, generator=g0).to(DEV)  # noqa: E731
@@ -382,8 +348,8 @@ def test_bn_bwd_routes_are_bit_equal():
 @pytest.mark.parametrize("C", [1, 2, 4, 8])
 def test_segloss_reduce_exact_sums(C, P):
     """logits equal within each pixel: p = 1/C exactly, so sum y, sum p*y and sum p*p are exact for integer y"""
-    _C, rt = _lib()
-    gen = _gen(C * P)
+    _C, rt = lib()
+    gen = dev_gen(C * P)
     logits = (torch.randn(P, 1, generator=gen, device=DEV) * 3).expand(P, C).contiguous()
     y = ints((P, C), 0, 3, gen)
     assert 32 * 3 < E.F32_EXACT
@@ -401,8 +367,8 @@ def test_segloss_reduce_exact_sums(C, P):
 @pytest.mark.parametrize("C", [2, 5, 8])
 def test_confusion_exact(C, P):
     """integer logits (many ties) and multi-hot labels (ties too): both argmaxes resolve to the first maximum"""
-    _C, rt = _lib()
-    gen = _gen(C + P)
+    _C, rt = lib()
+    gen = dev_gen(C + P)
     logits = ints((P, C), -2, 2, gen)
     y = ints((P, C), 0, 1, gen)
     counts = torch.zeros(C * C, dtype=torch.int64, device=DEV)
@@ -414,8 +380,8 @@ def test_confusion_exact(C, P):
 
 @pytest.mark.parametrize("n", [16 * 2048, 100003, 1])
 def test_l2_loss_exact(n):
-    _C, rt = _lib()
-    w = ints((n,), -8, 8, _gen(n))
+    _C, rt = lib()
+    w = ints((n,), -8, 8, dev_gen(n))
     out = torch.full((1,), 3.0, dtype=torch.float64, device=DEV)
     _C.call("pnp_l2_loss_acc", ptr(w), n, ptr(out), rt.stream())
     sync()
@@ -425,8 +391,8 @@ def test_l2_loss_exact(n):
 @pytest.mark.parametrize("B,F", [(16, 2048), (3, 1001), (1, 1)])
 def test_fc_exact(B, F):
     """out = x @ w; dx = dout * w; dw += x^T dout (accumulating into a non-zero dw)"""
-    _C, rt = _lib()
-    gen = _gen(B * F)
+    _C, rt = lib()
+    gen = dev_gen(B * F)
     x, w, dout = ints((B, F), -8, 8, gen), ints((F,), -8, 8, gen), ints((B,), -8, 8, gen)
     assert 64 * F < E.F32_EXACT and 64 * B < E.F32_EXACT
     out = torch.full((B,), float("nan"), device=DEV)
@@ -445,8 +411,8 @@ def test_fc_exact(B, F):
 @pytest.mark.parametrize("n", [16 * 2048, 1001, 1])
 @pytest.mark.parametrize("with_b", [True, False])
 def test_mean_combo_exact(n, with_b):
-    _C, rt = _lib()
-    gen = _gen(n)
+    _C, rt = lib()
+    gen = dev_gen(n)
     a, b = ints((n,), -8, 8, gen), ints((n,), -8, 8, gen)
     out = torch.full((1,), float("nan"), device=DEV)
     _C.call("pnp_mean_combo", ptr(a), 0.5, ptr(b) if with_b else None, -2.0, n, ptr(out), rt.stream())
@@ -462,7 +428,7 @@ def test_mean_combo_exact(n, with_b):
 def test_bn_training_real(M):
     """pnp_bn_finalize and pnp_bn_apply_fused (training, skip, leaky ReLU) from fp64 sums of randn z: mean, invstd, scale, shift,
     the moving averages (unbiased factor M / (M - 1), 1 at M = 1) and y within TAU; both launchers agree bit for bit"""
-    _C, rt = _lib()
+    _C, rt = lib()
     C = 64
     g0 = torch.Generator().manual_seed(M)
     f = lambda *s: torch.randn(*s, generator=g0).to(DEV)  # noqa: E731
@@ -496,7 +462,7 @@ def test_bn_training_real(M):
 def test_segloss_real(C, P):
     """randn logits, one-hot y: the four class sums, then _finalize from the kernel's own acc, then _bwd from the kernel's own
     coef, each within TAU of the fp64 value"""
-    _C, rt = _lib()
+    _C, rt = lib()
     g0 = torch.Generator().manual_seed(C * 7 + P)
     logits = (torch.randn(P, C, generator=g0) * 3).to(DEV)
     y = torch.nn.functional.one_hot(torch.randint(0, C, (P,), generator=g0), C).float().to(DEV)
@@ -535,7 +501,7 @@ def invstd_sweep_variances(n=1 << 20, seed=0):
 
 def test_bn_finalize_invstd_ulps():
     """invstd = rsqrtf + one Newton step against the correctly rounded 1 / sqrt(fl(var + eps)), over 2^20 variances"""
-    _C, rt = _lib()
+    _C, rt = lib()
     var = invstd_sweep_variances().to(DEV)
     C = var.numel()
     zero, one = torch.zeros(C, device=DEV), torch.ones(C, device=DEV)
@@ -582,7 +548,7 @@ def test_subnormal_activation_sign():
     """rn_bf16 sends 0 < y <= 2^-134 to a bf16 +0, so a consumer reading the sign from y_hi would take the y <= 0 slope there.
     The producers (pnp_bn_act_apply, pnp_bn_apply_fused, the wgmma fused epilogue) flush positive subnormal activations to
     +0, so the y and y_hi paths agree on everything they write."""
-    _C, rt = _lib()
+    _C, rt = lib()
     vals = torch.tensor(SIGN_VALUES, dtype=torch.float32)
     z = vals.repeat_interleave(4).reshape(-1, 4).to(DEV)
     M, C = z.shape
@@ -601,7 +567,7 @@ def test_subnormal_activation_sign():
         zero, one, mm = torch.zeros(C, device=DEV), torch.ones(C, device=DEV), torch.zeros(C, device=DEV)
         for name in ("pnp_bn_act_apply", "pnp_bn_apply_fused"):
             y = torch.empty(M, C, device=DEV)
-            hi, lo = _planes((M, C), 3)
+            hi, lo = empty_planes((M, C), 3)
             if name == "pnp_bn_act_apply":
                 want = want_z
                 _C.call(name, ptr(z), None, None, None, 0, 0, act, ptr(y), ptr(hi), ptr(lo), M, C, rt.stream())
@@ -612,7 +578,7 @@ def test_subnormal_activation_sign():
             sync()
             y = y.cpu()
             assert torch.equal(y.view(torch.int32), want.view(torch.int32)), "%s act %d: %s" % (name, act, y.cpu().tolist())
-            _assert_planes(name, hi, lo, want)
+            assert_planes(name, hi, lo, want)
             s = _slopes(_C, rt, y.to(DEV), hi, act)
             for k in (0, 1):
                 assert torch.equal(s["y"][k], s["y_hi"][k]), "%s act %d: the y and y_hi paths disagree" % (name, act)
@@ -621,9 +587,7 @@ def test_subnormal_activation_sign():
 
 def _tc_epilogue_sign(_C, rt, vals, act):
     """the wgmma fused epilogue: zero operands, shift = the edge values per channel, so y = act(shift)"""
-    from pnp_b200 import runtime as rt_mod
-    if not rt_mod.tc_available():
-        pytest.fail("wgmma path unavailable on this device")
+    lib(require_tc=True)
     B, H, W, Cin, Cout = 1, 8, 8, 64, 64
     x_hi = torch.zeros(B * H * W * Cin, dtype=torch.bfloat16, device=DEV)
     w_hi = torch.zeros(Cin * Cout, dtype=torch.bfloat16, device=DEV)
@@ -649,7 +613,7 @@ VAR_CASES = [(M, r) for M in (4, 32, 8192) for r in (0, 1, 10, 100)]
 def test_bn_variance_conditioning():
     """pnp_bn_stats + pnp_bn_finalize on z = r + N(0, 1): |var - var_ref| <= TAU * E[z^2] (one-pass variance); prints the
     relative error of invstd, which grows as (mean / std)^2"""
-    _C, rt = _lib()
+    _C, rt = lib()
     C = 64
     rows = []
     for M, r in VAR_CASES:
@@ -743,18 +707,18 @@ REJECT = _rejections()
 
 @pytest.mark.parametrize("i", range(len(REJECT)), ids=[r[0].replace(" ", "_") for r in REJECT])
 def test_rejected_calls_leave_outputs_untouched(i):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, build, code = REJECT[i]
     n = 8 * 1028
     b = {k: torch.full((n,), 1234.5, device=DEV) for k in ("z", "dy", "y", "c", "skip", "out", "mm", "mv", "mo", "io")}
     b.update({k: torch.full((n,), 1234.5, dtype=torch.float64, device=DEV) for k in ("s1", "s2", "s1c", "s2c")})
+    before = snapshot(b)
     name, args = build(b)
     args = args[:-1] + (rt.stream(),)
     rc = getattr(_C.lib, name)(*args)
     sync()
     assert rc == code, "%s: %s returned %d, expected %d" % (tag, name, rc, code)
-    for k, t in b.items():
-        assert bool((t == 1234.5).all()), "%s: %s wrote %s" % (tag, name, k)
+    assert_untouched(tag, name, b, before)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -762,12 +726,6 @@ def test_rejected_calls_leave_outputs_untouched(i):
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.timeout(300)
 def test_exact_cases_under_pdl():
-    env = dict(os.environ)
-    env["PNP_PDL"] = "1"
-    t0 = time.time()
-    p = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-s", "-p", "no:cacheprovider", os.path.abspath(__file__), "-k",
-                        "(bn_stats_exact or bwd_reduce_exact or act_apply_exact or apply_fused_exact or bwd_apply_exact) "
-                        "and not under_pdl"], cwd=ROOT, env=env, capture_output=True, text=True, timeout=280)
-    lines = p.stdout.splitlines()
-    print("  PNP_PDL=1: %s (wall %.1f s)" % (lines[-1] if lines else "", time.time() - t0))
-    assert p.returncode == 0, "\n".join(lines[-25:])
+    passed, _ = rerun({"PNP_PDL": "1"}, __file__, "(bn_stats_exact or bwd_reduce_exact or act_apply_exact or apply_fused_exact or "
+                      "bwd_apply_exact) and not under_pdl", flags=("-s",))
+    assert passed == 2 * len(REDUCE_CASES) + 3 * len(APPLY_SHAPES) + 6 * len(BWD_SHAPES), passed

@@ -15,7 +15,7 @@ import pytest
 import torch
 
 from tests.util import check
-from tests.test_parity_configs_gpu import loss_close, state_close, _bn_noise
+from tests.models import bn_noise, loss_close, state_close
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -65,7 +65,7 @@ def test_segmenter_checkpoint_hands_over_to_pretrain_discriminator_step(tmp_path
     # ---- phase 1: pre-train graph, the reference's restore chain ------------------------------------------------------
     ws, bns = OracleAdversarial.layout()
     Padv = init_numpy_params(ws, bns, 1, 0.05)            # a DIFFERENT seed: everything the chain must overwrite differs
-    _bn_noise(Padv, bns, 11)
+    bn_noise(Padv, bns, 11)
     for n, s in ws:
         if "cls" in n:
             Padv[n] = np.clip(Padv[n] * 0.5, -0.05, 0.05).astype(np.float32)
@@ -122,7 +122,7 @@ def test_evaluation_path_matches_oracle():
     rt.set_conv_backend("auto")
     ws, bns = OracleAdversarial.layout()
     P = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(P, bns, 6)
+    bn_noise(P, bns, 6)
     ck, nc, tc = configure("train-gan")
     net = adv.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=ck, network_config=nc)
     rt.load_state_dict(P)
@@ -163,7 +163,7 @@ def test_per_volume_evaluation_matches_oracle():
     rt.set_conv_backend("auto")
     ws, bns = OracleAdversarial.layout()
     P = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(P, bns, 6)
+    bn_noise(P, bns, 6)
     ck, nc, tc = configure("train-gan")
     net = adv.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=ck, network_config=nc)
     rt.load_state_dict(P)
@@ -221,7 +221,7 @@ def test_test_eval_on_nifti_subjects_both_trainers(tmp_path):
     # ---- adversarial trainer: the adapted CT stream -----------------------------------------------------------------
     ws, bns = OracleAdversarial.layout()
     P = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(P, bns, 6)
+    bn_noise(P, bns, 6)
     ck, nc, tc = configure("train-gan")
     net = adv.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=ck, network_config=nc)
     rt.load_state_dict(P)
@@ -250,7 +250,7 @@ def test_test_eval_on_nifti_subjects_both_trainers(tmp_path):
     # ---- segmenter trainer: frames in order --------------------------------------------------------------------------
     ws, bns = OracleSegmenter.layout()
     Ps = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(Ps, bns, 6)
+    bn_noise(Ps, bns, 6)
     snet = seg.Full_DRN(channels=3, n_class=5, batch_size=B,
                         cost_kwargs={"cross_flag": True, "miu_cross": 1.0, "dice_flag": True, "miu_dice": 1.0})
     rt.load_state_dict(Ps)

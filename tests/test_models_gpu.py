@@ -7,35 +7,15 @@ synthetic 256x256x3 inputs and identical initial variables (loaded by TF variabl
 Tolerance (BASELINE.json north_star): 1e-3 relative fp32, stated per check; dropout off (keep_prob=1,
 critic_keep_prob=1) because TF's Philox stream cannot be reproduced (SURVEY App. B.4).
 """
-import numpy as np
 import pytest
 import torch
 
+from tests.models import adv_pair, seg_pair, state_close
 from tests.util import check, rel_err, l2_err
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 B = 2
-
-
-def _seg_pair(backend, dtype=torch.float32):
-    import pnp_b200
-    from pnp_b200 import runtime as rt, source_segmenter as seg
-    from oracle.pnp_graphs import OracleSegmenter, init_numpy_params
-    rt.set_conv_backend(backend)
-    ws, bns = OracleSegmenter.layout()
-    P = init_numpy_params(ws, bns, 0, 0.05)
-    rng = np.random.RandomState(5)
-    for n, c in bns:   # non-trivial BN state so that inference-mode BN is really exercised
-        P[n + "/gamma"] = (1 + 0.2 * rng.randn(c)).astype(np.float32)
-        P[n + "/beta"] = (0.1 * rng.randn(c)).astype(np.float32)
-        P[n + "/moving_mean"] = (0.05 * rng.randn(c)).astype(np.float32)
-        P[n + "/moving_variance"] = (1 + 0.2 * rng.rand(c)).astype(np.float32)
-    ck = {"cross_flag": True, "miu_cross": 1.0, "dice_flag": True, "miu_dice": 1.0, "regularizer": 1e-4}
-    net = seg.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=dict(ck))
-    rt.load_state_dict(P)
-    oracle = OracleSegmenter(P, B, dtype=dtype)
-    return net, oracle, P
 
 
 def _inputs():
@@ -51,7 +31,7 @@ def _inputs():
 @pytest.mark.parametrize("bn_train", [True, False])
 def test_config1_segmenter_forward(backend, bn_train):
     from pnp_b200 import runtime as rt
-    net, oracle, _ = _seg_pair(backend)
+    net, _, oracle, _ = seg_pair(backend, B)
     x, lab, y = _inputs()
     with torch.no_grad():
         ref = oracle.forward(x, 1.0, bn_train)
@@ -74,10 +54,9 @@ def test_config1_segmenter_forward(backend, bn_train):
 
 @pytest.mark.parametrize("backend", ["simt", "auto"])
 def test_config2_segmenter_train_step(backend):
-    from pnp_b200 import runtime as rt, source_segmenter as seg
-    net, oracle, P = _seg_pair(backend)
+    from pnp_b200 import runtime as rt
+    net, trainer, oracle, P = seg_pair(backend, B)
     x, lab, y = _inputs()
-    trainer = seg.Trainer(net, [], [], num_cls=5, batch_size=B, optimizer="adam", opt_kwargs={"learning_rate": 1e-3})
     xg, yg = trainer.feed(x, torch.from_numpy(lab))
     assert torch.equal(yg.cpu(), y)
     from oracle.pnp_graphs import OracleSegmenter
@@ -99,18 +78,10 @@ def test_config2_segmenter_train_step(backend):
                 mult = sum(1 for w in net.conv_weights if w is v)
                 ours.append(v.grad.cpu().double() + 1e-4 * mult * torch.tensor(P[n]).double())
             _grad_report(all_names, ours, ro["grads"], g64, slack=4.0 if backend == "simt" else 10.0)
-    ref = oracle.ps.to_numpy()
-    got = rt.state_dict()
-    worst, wname = 0.0, None
-    for n in ref:
-        e = l2_err(torch.tensor(got[n]), torch.tensor(ref[n]))
-        if e > worst:
-            worst, wname = e, n
-    print("  worst variable after 2 Adam steps: %s l2 err %.3e" % (wname, worst))
     # Adam's first updates are ~ lr*sign(g): elements whose gradient sits below the fp32 noise floor of this backward pass
     # (see _grad_report) may step the other way, so variables are compared in relative L2 (a few 1e-3 of the elements
     # moving by 2*lr), not max-norm; the per-step losses above are the end-to-end check at 1e-3
-    assert worst <= 2e-2
+    state_close(rt, oracle, 2e-2, norm=l2_err, label="worst variable after 2 Adam steps: {name} l2 err {err:.3e}")
     reg = net.regularizer_loss()
     assert abs(reg - float(oracle.losses(oracle.forward(x, 1.0, False)["logits"], y)[1])) <= 1e-3 * abs(reg)
     rt.set_conv_backend("auto")
@@ -128,34 +99,6 @@ def _grad_report(names, ours, g32, g64, slack=4.0, floor=2e-3):
         wp, wo = max(wp, ep), max(wo, eo)
     print("  worst gradient l2 err vs fp64 oracle: ours %.3e, fp32 oracle %.3e" % (wp, wo))
     assert wp <= slack * wo + floor, (wp, wo)
-
-
-def _adv_pair(backend, lam, phase):
-    import pnp_b200
-    from pnp_b200 import runtime as rt, adversarial as adv
-    from pnp_b200.train_gan import configure
-    from oracle.pnp_graphs import OracleAdversarial, init_numpy_params
-    rt.set_conv_backend(backend)
-    ws, bns = OracleAdversarial.layout()
-    P = init_numpy_params(ws, bns, 0, 0.05)
-    rng = np.random.RandomState(6)
-    for n, c in bns:
-        P[n + "/gamma"] = (1 + 0.2 * rng.randn(c)).astype(np.float32)
-        P[n + "/beta"] = (0.1 * rng.randn(c)).astype(np.float32)
-        P[n + "/moving_mean"] = (0.05 * rng.randn(c)).astype(np.float32)
-        P[n + "/moving_variance"] = (1 + 0.2 * rng.rand(c)).astype(np.float32)
-    for n, s in ws:   # keep the critic weights inside the clip range so the clip is exercised but not dominant
-        if "cls" in n:
-            P[n] = np.clip(P[n] * 0.5, -0.05, 0.05).astype(np.float32)
-    ck, nc, tc = configure(phase)
-    ck["lambda_mask_loss"] = lam
-    tc["dis_sub_iter"] = 3
-    net = adv.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=ck, network_config=nc, critic_keep_prob=1.0)
-    rt.load_state_dict(P)
-    trainer = adv.Trainer(net, num_cls=5, batch_size=B, opt_kwargs={"learning_rate": 3e-4}, train_config=tc)
-    oracle = OracleAdversarial(P, B, lambda_mask_loss=lam, dis_sub_iter=3, gen_sub_iter=1, critic_keep_prob=1.0)
-    oracle.o64 = OracleAdversarial(P, B, dtype=torch.float64, lambda_mask_loss=lam, dis_sub_iter=3, gen_sub_iter=1, critic_keep_prob=1.0)
-    return net, trainer, oracle
 
 
 def _compare_grads(rt, oracle, which, g32, g64, backend="simt"):
@@ -188,25 +131,11 @@ def _snapshot(rt):
         PRE[n] = rt.graph.vars[n].detach().cpu().clone()
 
 
-def _compare_state(rt, oracle, tol, only=None):
-    ref = oracle.ps.to_numpy()
-    got = rt.state_dict()
-    worst, wname = 0.0, None
-    for n in ref:
-        if only and not only(n):
-            continue
-        e = rel_err(torch.tensor(got[n]), torch.tensor(ref[n]))
-        if e > worst:
-            worst, wname = e, n
-    print("  worst variable: %s rel err %.3e" % (wname, worst))
-    assert worst <= tol, (wname, worst)
-
-
 @pytest.mark.parametrize("backend", ["simt", "auto"])
 def test_config3_discriminator_pretrain_step(backend):
     from pnp_b200 import runtime as rt
     from oracle.pnp_graphs import synthetic_images
-    net, trainer, oracle = _adv_pair(backend, 0, "pre-train")
+    net, trainer, oracle = adv_pair(backend, 0, "pre-train", B, dis_sub_iter=3, o64=True)
     mr, ct = synthetic_images(B, 1234), synthetic_images(B, 4321, 0.3, 0.8)
     for step in range(2):
         _snapshot(rt)
@@ -217,7 +146,7 @@ def test_config3_discriminator_pretrain_step(backend):
         got = trainer.loss_value(terms)
         print("  step %d dis_loss %.6e (oracle %.6e)" % (step, got, ro["dis_loss"]))
         assert abs(got - ro["dis_loss"]) <= 1e-3 * max(abs(ro["dis_loss"]), 2e-3 * float(ro["mr_cls"].abs().max()))
-    _compare_state(rt, oracle, 1e-3)
+    state_close(rt, oracle, 1e-3, label="worst variable: {name} rel err {err:.3e}")
     check("dis_reg", torch.tensor([net.dis_reg()]), torch.tensor([float(oracle.dis_losses(ro["ct_cls"], ro["mr_cls"], None, None)[1])]), 1e-3)
     rt.set_conv_backend("auto")
 
@@ -226,7 +155,7 @@ def test_config3_discriminator_pretrain_step(backend):
 def test_config4_joint_adversarial_step(backend):
     from pnp_b200 import runtime as rt
     from oracle.pnp_graphs import synthetic_images
-    net, trainer, oracle = _adv_pair(backend, 0.3, "train-gan")
+    net, trainer, oracle = adv_pair(backend, 0.3, "train-gan", B, dis_sub_iter=3, o64=True)
     mr, ct = synthetic_images(B, 1234), synthetic_images(B, 4321, 0.3, 0.8)
     _snapshot(rt)
     ro = oracle.d_step(mr, ct, keep_prob=1.0)
@@ -242,7 +171,7 @@ def test_config4_joint_adversarial_step(backend):
     got = trainer.loss_value(terms)
     print("  gen_loss %.6e (oracle %.6e)" % (got, rg["gen_loss"]))
     assert abs(got - rg["gen_loss"]) <= 1e-3 * max(abs(rg["gen_loss"]), 2e-3 * float(rg["ct_cls"].abs().max()))
-    _compare_state(rt, oracle, 1e-3)
+    state_close(rt, oracle, 1e-3, label="worst variable: {name} rel err {err:.3e}")
     rt.set_conv_backend("auto")
 
 
@@ -254,7 +183,7 @@ def test_cuda_graph_replay_equals_eager_steps():
     mr, ct = synthetic_images(B, 1234).to(DEV), synthetic_images(B, 4321, 0.3, 0.8).to(DEV)
     states = []
     for use_graph in (False, True):
-        net, trainer, _ = _adv_pair("simt", 0.3, "train-gan")
+        net, trainer, _ = adv_pair("simt", 0.3, "train-gan", B, dis_sub_iter=3, o64=True)
         if use_graph:
             assert trainer.capture_joint_step(mr, ct, keep_prob=1.0, warmup=1), "CUDA-graph capture failed"
             for _ in range(2):

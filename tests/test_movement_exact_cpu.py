@@ -16,6 +16,7 @@ from oracle import pnp_graphs as PG
 from oracle import tf14_numpy as N
 from oracle import tf14_torch as T
 from tests import test_movement_exact_gpu as G
+from tests.cabi import sentinel
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CPU = "cpu"
@@ -345,7 +346,7 @@ def _margin_ps(bwd, **bug):
         if bwd:
             d += ndiff(M.phase_shift_bwd_ref(dout, r, G_, coff, ntile, o, **bug), M.phase_shift_bwd_ref(dout, r, G_, coff, ntile, o))
         else:
-            base = G.sentinel((B, a * r, b * r, Ctot), CPU)
+            base = sentinel((B, a * r, b * r, Ctot), CPU)
             d += ndiff(M.phase_shift_fwd_ref(X, base, r, G_, coff, ntile, o, **bug), M.phase_shift_fwd_ref(X, base, r, G_, coff,
                                                                                                            ntile, o))
     return d
@@ -364,7 +365,7 @@ def _margin_lac():
     d = 0
     for tag, P, C, Ctot, coff in small(G.LAC_CASES):
         logits = G.small_ints((P, C), P + C, -1, 1, CPU)
-        base = G.sentinel((P, Ctot), CPU)
+        base = sentinel((P, Ctot), CPU)
         d += ndiff(M.logits_argmax_concat_ref(logits, base, coff, last=True), M.logits_argmax_concat_ref(logits, base, coff))
     return d + _margin_disc(last=True)
 
@@ -385,7 +386,7 @@ def _margin_slice():
     d = 0
     for tag, Mr, C, off, Cs, acc in small(G.SLICE_CASES):
         g = G.operand("randn", (Mr, C), Mr + C, CPU)
-        out = G.operand("randn", (Mr, Cs), 3 * Mr + Cs, CPU) if acc else G.sentinel((Mr, Cs), CPU)
+        out = G.operand("randn", (Mr, Cs), 3 * Mr + Cs, CPU) if acc else sentinel((Mr, Cs), CPU)
         d += ndiff(M.channel_slice_ref(g, C, off, Cs, out, acc, ignore_acc=True), M.channel_slice_ref(g, C, off, Cs, out, acc))
     return d
 
@@ -396,7 +397,7 @@ def _margin_one_hot():
 
 
 def _margin_fill():
-    return sum(ndiff(M.fill_ref(G.sentinel(n + 5, CPU), -3.25, n, drop_tail=True), M.fill_ref(G.sentinel(n + 5, CPU), -3.25, n))
+    return sum(ndiff(M.fill_ref(sentinel(n + 5, CPU), -3.25, n, drop_tail=True), M.fill_ref(sentinel(n + 5, CPU), -3.25, n))
                for n in G.FILL_N if n < 10 ** 6)
 
 

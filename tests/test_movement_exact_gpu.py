@@ -12,21 +12,15 @@ c. the functional fallback route of the discriminator input (a channel count tha
 d. rejected calls return PNP_ERR_BAD_ARG / PNP_ERR_UNSUPPORTED and leave every output untouched;
 e. the exact cases again under PNP_PDL=1, in their own process."""
 import ctypes
-import os
-import subprocess
-import sys
-import time
 
 import pytest
 import torch
 
 from oracle import movement_exact as M
+from tests.cabi import (BAD_ARG, DEV, SENTINEL, UNSUPPORTED, assert_bits, assert_untouched, cpu_gen, ints, lib, pick, ptr, rerun,
+                        sentinel, snapshot, sync)
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEV = "cuda"
-BAD_ARG, UNSUPPORTED = 100001, 100002
-SENTINEL = 0x7FC0BEEF           # a quiet NaN no kernel computes
 INF = float("inf")
 
 # ------------------------------------------------------------------------------------------------
@@ -100,57 +94,18 @@ def ids(cases):
 # ------------------------------------------------------------------------------------------------
 # helpers
 # ------------------------------------------------------------------------------------------------
-def _lib():
-    import pnp_b200  # noqa: F401
-    from pnp_b200 import _C, runtime as rt
-    return _C, rt
-
-
-def ptr(t):
-    return None if t is None else t.data_ptr()
-
-
-def sync():
-    torch.cuda.synchronize()
-
-
-def sentinel(shape, dev=DEV):
-    return torch.full(shape if isinstance(shape, tuple) else (shape,), SENTINEL, dtype=torch.int32, device=dev).view(torch.float32)
-
-
-def assert_bits(tag, got, ref):
-    g = got.contiguous().view(torch.int32).reshape(-1)
-    r = ref.float().contiguous().view(torch.int32).reshape(-1)
-    assert g.shape == r.shape, (tag, tuple(got.shape), tuple(ref.shape))
-    bad = (g != r).nonzero()
-    if bad.numel():
-        i = int(bad[0])
-        raise AssertionError("%s: %d of %d elements differ; first at flat %d: got %r (0x%08x), ref %r (0x%08x)" % (
-            tag, bad.numel(), g.numel(), i, float(got.reshape(-1)[i]), int(g[i]) & 0xFFFFFFFF, float(ref.reshape(-1)[i]),
-            int(r[i]) & 0xFFFFFFFF))
-
-
-def _gen(seed):
-    return torch.Generator().manual_seed(seed)
-
-
-def _pick(shape, values, gen):
-    v = torch.tensor(values, dtype=torch.float32)
-    return v[torch.randint(0, len(values), shape, generator=gen)]
-
-
 def operand(kind, shape, seed, dev=DEV):
     """the pooling operands.  ints: integers in [-2, 2]; const: one integer per (image, channel) plane; inf: +-inf, +-FLT_MAX and
     small integers; neginf: mostly -inf (many windows are all -inf); randn.  None holds -0.0."""
-    g = _gen(seed)
+    g = cpu_gen(seed)
     if kind == "ints":
         v = torch.randint(-2, 3, shape, generator=g).float()
     elif kind == "const":
         v = torch.randint(-2, 3, (shape[0], 1, 1, shape[3]), generator=g).float().expand(*shape).contiguous()
     elif kind == "inf":
-        v = _pick(shape, [-INF, INF, -M.FLT_MAX, M.FLT_MAX, -1.0, 1.0, 2.0], g)
+        v = pick(shape, [-INF, INF, -M.FLT_MAX, M.FLT_MAX, -1.0, 1.0, 2.0], g)
     elif kind == "neginf":
-        v = _pick(shape, [-INF] * 6 + [0.0, 1.0], g)
+        v = pick(shape, [-INF] * 6 + [0.0, 1.0], g)
     elif kind == "randn":
         v = torch.randn(shape, generator=g)
     else:
@@ -167,7 +122,7 @@ def distinct(shape, dev=DEV, offset=1):
 
 
 def small_ints(shape, seed, lo=-8, hi=8, dev=DEV):
-    return torch.randint(lo, hi + 1, shape, generator=_gen(seed)).float().to(dev)
+    return ints(shape, lo, hi, cpu_gen(seed)).to(dev)
 
 
 def ps_operands(case, dev=DEV):
@@ -186,7 +141,7 @@ def disc_operands(case, dev=DEV):
 
 def one_hot_labels(P, C, seed, dev=DEV):
     vals = torch.tensor([-1, C, 1 << 40, -(1 << 40)] + list(range(C)), dtype=torch.int64)
-    return vals[torch.randint(0, len(vals), (P,), generator=_gen(seed))].to(dev)
+    return vals[torch.randint(0, len(vals), (P,), generator=cpu_gen(seed))].to(dev)
 
 
 def _launch_note(tag, launch):
@@ -199,7 +154,7 @@ def _launch_note(tag, launch):
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("case", MAXPOOL2_CASES, ids=ids(MAXPOOL2_CASES))
 def test_maxpool2_exact(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, B, H, W, C, kind = case
     V, launch = M.maxpool2_launch(B, H, W, C)
     _launch_note("%s V=%d" % (tag, V), launch)
@@ -218,7 +173,7 @@ def test_maxpool2_exact(case):
 @pytest.mark.parametrize("case", MAXPOOL2_CASES, ids=ids(MAXPOOL2_CASES))
 def test_avgpool2_exact(case):
     """integer operands: the fp32 window sum is exact and 0.25f * sum = sum / 4; the backward 0.25f * dy is exact for any dy"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, B, H, W, C, _ = case
     _launch_note(tag, M.avgpool2_launch(B, H, W, C))
     x = operand("ints", (B, H, W, C), 3 + B + H)
@@ -236,7 +191,7 @@ def test_avgpool2_exact(case):
 @pytest.mark.parametrize("case", POOL_CASES, ids=ids(POOL_CASES))
 def test_pool_exact(case):
     """pnp_pool_fwd / _bwd, max and average: bit for bit (average on integer operands; its backward with x = NULL)"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, B, H, W, C, n, kind = case
     Ho, Wo, pt, pl = M.pool_geom(H, W, n)
     _launch_note(tag + " fwd", M.pool_launch(B, H, W, C, n, False))
@@ -266,10 +221,10 @@ def test_pool_exact(case):
 def test_maxpool_signed_zero_tie():
     """windows of +0.0 and -0.0 only: the max compares equal to 0 (which zero fmaxf returns is not pinned) and the gradient goes
     to the window's first element"""
-    _C, rt = _lib()
+    _C, rt = lib()
     for C, n in ((4, 2), (3, 2), (2, 3)):
         B, H, W = 2, 6, 6
-        x = _pick((B, H, W, C), [0.0, -0.0], _gen(C + n)).to(DEV)
+        x = pick((B, H, W, C), [0.0, -0.0], cpu_gen(C + n)).to(DEV)
         Ho, Wo, _, _ = M.pool_geom(H, W, n)
         dy = distinct((B, Ho, Wo, C))
         for fwd, bwd, extra in (("pnp_maxpool2_fwd", "pnp_maxpool2_bwd", ()), ("pnp_pool_fwd", "pnp_pool_bwd", (n, 0))):
@@ -288,7 +243,7 @@ def test_maxpool_signed_zero_tie():
                          ids=lambda c: c[0])
 def test_avg_pool_real(case):
     """randn: |y - y64| <= gamma_k * sum|x| / k for a window of k valid elements (k - 1 additions and one division)"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, B, H, W, C, n = case
     x = operand("randn", (B, H, W, C), 21 + n)
     Ho, Wo, _, _ = M.pool_geom(H, W, n)
@@ -310,7 +265,7 @@ def test_avg_pool_real(case):
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("case", MIRROR_CASES, ids=ids(MIRROR_CASES))
 def test_mirror_pad_exact(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, B, H, W, C, p = case
     _launch_note(tag + " fwd", M.mirror_pad_launch(B, H, W, C, p, False))
     _launch_note(tag + " bwd", M.mirror_pad_launch(B, H, W, C, p, True))
@@ -329,7 +284,7 @@ def test_mirror_pad_exact(case):
 @pytest.mark.parametrize("case", [c for c in MIRROR_CASES if c[0] != "cap"], ids=[c[0] for c in MIRROR_CASES if c[0] != "cap"])
 def test_mirror_pad_bwd_real(case):
     """randn dy: |dx - dx64| <= gamma_k * sum|terms| for an element that sums k padded positions"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, B, H, W, C, p = case
     dy = operand("randn", (B, H + 2 * p, W + 2 * p, C), 33 + p)
     dx = sentinel((B, H, W, C))
@@ -347,7 +302,7 @@ def test_mirror_pad_bwd_real(case):
 @pytest.mark.parametrize("case", PS_CASES, ids=ids(PS_CASES))
 def test_phase_shift_exact(case):
     """forward into a sentinel tensor: channels outside [coff, coff + ntile*G) keep the sentinel; backward sums the ntile copies"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, B, a, b, G, r, Ctot, coff, ntile, o = case
     _launch_note(tag, M.phase_shift_launch(B, a, b, G, r))
     X, dout = ps_operands(case)
@@ -372,7 +327,7 @@ def _disc_call(_C, rt, srcs, Gs, nts, logits, out, B, a, b, r, o):
 
 @pytest.mark.parametrize("case", DISC_CASES, ids=ids(DISC_CASES))
 def test_disc_input_exact(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, B, a, b, r, o, Gs, nts, NC = case
     path, launch = M.disc_input_launch(B, a, b, r, o, Gs, nts, NC)
     _launch_note("%s %s" % (tag, path), launch)
@@ -390,7 +345,7 @@ def test_disc_input_functional_fallback(B, o):
     """functional.disc_input with 4 logits channels: Ctot = 31 is not a multiple of 4, so the layer runs pnp_phase_shift_fwd per
     source and pnp_logits_argmax_concat; forward bit for bit, backward (pnp_phase_shift_bwd with ntile 3, pnp_channel_slice)
     bit for bit on integer dout"""
-    _lib()
+    lib()
     from pnp_b200 import functional as F
     a = b = 2
     r, Gs, nts, NC = 8, (2, 4, 8, 8), (3, 1, 1, 1), 4
@@ -416,7 +371,7 @@ def test_disc_input_functional_fallback(B, o):
 @pytest.mark.parametrize("case", LAC_CASES, ids=ids(LAC_CASES))
 def test_logits_argmax_concat_exact(case):
     """channels outside [coff, coff + C] keep the sentinel; argmax takes the lowest index on ties"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, P, C, Ctot, coff = case
     _launch_note(tag, M.pixel_launch(P))
     logits = small_ints((P, C), P + C, -1, 1)
@@ -429,7 +384,7 @@ def test_logits_argmax_concat_exact(case):
 
 @pytest.mark.parametrize("case", SLICE_CASES, ids=ids(SLICE_CASES))
 def test_channel_slice_exact(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, Mr, C, off, Cs, acc = case
     _launch_note(tag, M.channel_slice_launch(Mr, Cs))
     g = operand("randn", (Mr, C), Mr + C)
@@ -445,7 +400,7 @@ def test_channel_slice_exact(case):
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("case", CAT_CASES, ids=ids(CAT_CASES))
 def test_crop_concat_exact(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, B, H1, W1, C1, H2, W2, C2, w1, w2 = case
     _launch_note(tag + " fwd", M.crop_concat_launch(B, H1, W1, C1, H2, W2, C2, False))
     _launch_note(tag + " bwd", M.crop_concat_launch(B, H1, W1, C1, H2, W2, C2, True, w1, w2))
@@ -469,7 +424,7 @@ def test_crop_concat_exact(case):
 @pytest.mark.parametrize("case", ONE_HOT_CASES, ids=ids(ONE_HOT_CASES))
 def test_one_hot_exact(case):
     """labels -1, C, 2^40 and -2^40 give a zero row"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, P, C = case
     _launch_note(tag, M.pixel_launch(P))
     labels = one_hot_labels(P, C, P + C)
@@ -482,7 +437,7 @@ def test_one_hot_exact(case):
 @pytest.mark.parametrize("n", FILL_N)
 def test_fill_exact(n):
     """the n % 4 tail is written by CTA 0; nothing past n is touched"""
-    _C, rt = _lib()
+    _C, rt = lib()
     fl = M.fill_launch(n)
     print("  n %d grid %d capped %d iters %d tail %d" % (n, fl.grid, fl.capped, fl.iters, fl.tail))
     buf = sentinel(n + 5)
@@ -497,7 +452,7 @@ def test_fill_exact(n):
 # ------------------------------------------------------------------------------------------------
 def ps2_logits(P, C, seed, dev=DEV):
     """randn * 3 logits, with every 97th pixel at -200 + c (every expf underflows) and every 89th at 89 + c (expf overflows)"""
-    l = (torch.randn((P, C), generator=_gen(seed)) * 3).float()
+    l = (torch.randn((P, C), generator=cpu_gen(seed)) * 3).float()
     l[::97] = -200.0 + torch.arange(C, dtype=torch.float32)
     l[1::89] = 89.0 + torch.arange(C, dtype=torch.float32)
     return l.to(dev)
@@ -506,7 +461,7 @@ def ps2_logits(P, C, seed, dev=DEV):
 @pytest.mark.parametrize("case", PS2_CASES, ids=ids(PS2_CASES))
 def test_pixel_softmax2(case):
     """|p - p64| <= ps2_bound(C) * p64 per element; the underflow and overflow pixels are -1e15f exactly"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, P, C = case
     _launch_note(tag, M.pixel_launch(P))
     l = ps2_logits(P, C, P + C)
@@ -527,7 +482,7 @@ def test_pixel_softmax2(case):
 
 def ce_operands(n, seed, dev=DEV):
     """y in [0, 1) at multiples of 1/8, p = 2^-k (k in 0..20) with a few p outside [1e-10, 1] and at its ends"""
-    g = _gen(seed)
+    g = cpu_gen(seed)
     y = (torch.randint(0, 8, (n,), generator=g).float() / 8)
     p = torch.pow(2.0, -torch.randint(0, 21, (n,), generator=g).float())
     special = torch.tensor([1.0, 2.0, 1e-11, 0.0, -1.0, 1.5], dtype=torch.float32)
@@ -542,7 +497,7 @@ def ce_operands(n, seed, dev=DEV):
 def test_cross_entropy_bwd(n):
     """dp bit for bit (dyadic y, power-of-two p, k = -g/n = -1/2 exact) and 0 outside [1e-10, 1]; dy = k log(clip p) within
     CE_DY_BOUND (0 exactly at p = 1)"""
-    _C, rt = _lib()
+    _C, rt = lib()
     _launch_note("n %d" % n, M.ce_bwd_launch(n))
     y, p = ce_operands(n, n)
     g = torch.tensor([0.5 * n], dtype=torch.float32, device=DEV)
@@ -562,9 +517,9 @@ def test_cross_entropy_bwd(n):
 
 def test_cross_entropy_bwd_real():
     """randn-derived y and p in (0, 1.5), an inexact k: dy within CE_DY_BOUND, dp within CE_DP_BOUND; one output NULL at a time"""
-    _C, rt = _lib()
+    _C, rt = lib()
     n = 100003
-    g = _gen(5)
+    g = cpu_gen(5)
     y = torch.rand((n,), generator=g).to(DEV)
     p = torch.rand((n,), generator=g) * 1.5
     p[:3] = torch.tensor([M.CE_CLIP_LO, 1.0, 1e-12])
@@ -585,12 +540,12 @@ def test_cross_entropy_bwd_real():
 def test_cross_entropy_fwd(n):
     """acc (caller-zeroed) receives sum y log(clip p) within ce_acc_bound(n) * sum|y log clip p|; out = fl32(-acc / n) of the
     kernel's own acc.  A second call without re-zeroing adds the same sum again."""
-    _C, rt = _lib()
+    _C, rt = lib()
     launch = M.ce_acc_launch(n)
     _launch_note("n %d" % n, launch)
     y, p = ce_operands(n, n + 1)
     if n > 1:
-        y = y + torch.rand((n,), generator=_gen(n)).to(DEV) / 8        # inexact terms
+        y = y + torch.rand((n,), generator=cpu_gen(n)).to(DEV) / 8        # inexact terms
     ref, mag = M.cross_entropy_fwd_ref(y, p)
     acc = torch.zeros(1, dtype=torch.float64, device=DEV)
     out = sentinel(1)
@@ -705,37 +660,29 @@ def _buffers():
     return b
 
 
-def _untouched(tag, name, b):
-    for k, t in b.items():
-        if k == "lab":
-            assert bool((t == 0).all()), "%s: %s wrote labels" % (tag, name)
-        elif t.dtype == torch.float64:
-            assert bool((t == 1234.5).all()), "%s: %s wrote %s" % (tag, name, k)
-        else:
-            assert bool((t.view(torch.int32) == SENTINEL).all()), "%s: %s wrote %s" % (tag, name, k)
-
-
 @pytest.mark.parametrize("i", range(len(REJECT)), ids=[r[0].replace(" ", "_") for r in REJECT])
 def test_rejected_calls_leave_outputs_untouched(i):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, build, code = REJECT[i]
     b = _buffers()
+    before = snapshot(b)
     name, args = build(b)
     sync()
     rc = getattr(_C.lib, name)(*(args + (rt.stream(),)))
     sync()
     assert rc == code, "%s: %s returned %d, expected %d" % (tag, name, rc, code)
-    _untouched(tag, name, b)
+    assert_untouched(tag, name, b, before)
 
 
 @pytest.mark.parametrize("i", range(len(DISC_REJECT)), ids=[r[0].replace(" ", "_") for r in DISC_REJECT])
 def test_disc_input_rejections(i):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, o, code = DISC_REJECT[i]
     B, r, G, nt, NC = o.get("B", 2), o.get("r", 4), o.get("G", (2, 4)), o.get("nt", (3, 1)), o.get("NC", 5)
     H, W = o.get("H", 4), o.get("W", 4)
     nsrc = o.get("nsrc", 2)
     b = _buffers()
+    before = snapshot(b)
     srcs = (ctypes.c_void_p * 5)(*([ptr(b["x"]), ptr(b["x2"])] * 3)[:5])
     if "null_src" in o:
         srcs[o["null_src"]] = None
@@ -746,12 +693,12 @@ def test_disc_input_rejections(i):
                                    B, H, W, r, 0, rt.stream())
     sync()
     assert rc == code, "%s: pnp_disc_input_fwd returned %d, expected %d" % (tag, rc, code)
-    _untouched(tag, "pnp_disc_input_fwd", b)
+    assert_untouched(tag, "pnp_disc_input_fwd", b, before)
 
 
 def test_disc_input_rejects_the_32bit_index_limit():
     """B * H * W * 64 >= 2^31 pixels-times-64 is UNSUPPORTED (the kernels index in 32 bits), with real buffers of that size"""
-    _C, rt = _lib()
+    _C, rt = lib()
     H = W = 5793                                  # 5793^2 * 64 >= 2^31
     assert H * W * 64 >= 1 << 31 and H * W * 4 < 1 << 31
     src = sentinel(H * W)
@@ -774,11 +721,6 @@ PDL_SELECTION = " or ".join(["maxpool2_exact", "avgpool2_exact", "test_pool_exac
 
 @pytest.mark.timeout(600)
 def test_exact_cases_under_pdl():
-    env = dict(os.environ)
-    env["PNP_PDL"] = "1"
-    t0 = time.time()
-    p = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-s", "-p", "no:cacheprovider", os.path.abspath(__file__), "-k",
-                        PDL_SELECTION], cwd=ROOT, env=env, capture_output=True, text=True, timeout=580)
-    lines = p.stdout.splitlines()
-    print("  PNP_PDL=1: %s (wall %.1f s)" % (lines[-1] if lines else "", time.time() - t0))
-    assert p.returncode == 0, "\n".join(lines[-25:])
+    passed, _ = rerun({"PNP_PDL": "1"}, __file__, PDL_SELECTION, flags=("-s",), timeout=580)
+    assert passed == (2 * len(MAXPOOL2_CASES) + len(POOL_CASES) + 1 + len(MIRROR_CASES) + len(PS_CASES) + len(DISC_CASES) + 2 +
+                      len(LAC_CASES) + len(SLICE_CASES) + len(CAT_CASES) + len(ONE_HOT_CASES) + len(FILL_N)), passed

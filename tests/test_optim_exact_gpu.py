@@ -13,20 +13,13 @@ e. rejected calls return PNP_ERR_BAD_ARG and leave every buffer untouched;
 f. the exact cases and the graph again under PNP_PDL=1, in their own process.
 
 Each real-valued test prints its worst ratio |got - ref| / magnitude next to TAU."""
-import ctypes
-import os
-import subprocess
-import sys
-
 import pytest
 import torch
 
 from oracle import optim_exact as O
+from tests.cabi import BAD_ARG, DEV, assert_untouched, lib, ptr, rerun, snapshot
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEV = "cuda"
-BAD_ARG = 100001
 
 # (id, optimizer, n, segments, grad_scale, segments with g = 0, monotone chunk_seg).  The CPU file maps each to what it reaches.
 EXACT_CASES = [
@@ -43,16 +36,6 @@ EXACT_CASES = [
     ("mom_2p24", "momentum", 1 << 24, 301, 1.0, 3, False),
 ]
 ARENA_SIZES = [1, 1023, 1024, 1025, 3 * 3 * 512 * 512]
-
-
-def _lib():
-    import pnp_b200  # noqa: F401
-    from pnp_b200 import _C, runtime as rt
-    return _C, rt
-
-
-def ptr(t):
-    return None if t is None else t.data_ptr()
 
 
 def dev(c):
@@ -85,7 +68,7 @@ def scalars(kind, c):
 
 
 def run_exact(kind, c, tag, with_clip=True):
-    _C, rt = _lib()
+    _C, rt = lib()
     cc = dict(c) if with_clip else {k: v for k, v in c.items() if k != "seg_clip"}
     ref = O.reference(kind, cc)
     outs = O.OUTPUTS[kind]
@@ -120,7 +103,7 @@ def test_step_exact(case):
 
 def test_adam_advance_matches_double():
     """state after t = 1 .. 50 advances equals the Python double computation bit for bit (betas promoted from fp32)"""
-    _C, rt = _lib()
+    _C, rt = lib()
     for b1, b2, lr in ((0.9, 0.999, 1e-3), (0.5, 0.75, 2e-4), (0.99, 0.9999, 0.1)):
         st = [1.0, 1.0, lr, 0.0]
         state_t = torch.tensor(st, dtype=torch.float64, device=DEV)
@@ -166,7 +149,7 @@ REAL = [("adam", 0.0), ("rmsprop", 0.0), ("rmsprop", 0.9), ("momentum", 0.2)]
 @pytest.mark.parametrize("kind,momentum", REAL, ids=["adam", "rmsprop_mom0", "rmsprop_mom09", "momentum"])
 def test_step_real(kind, momentum):
     """five steps from a randn state; each compared per element with the reference from the kernel's own previous state"""
-    _C, rt = _lib()
+    _C, rt = lib()
     c = real_case(kind, momentum, seed=17)
     d = dev(c)
     worst = 0.0
@@ -196,7 +179,7 @@ def test_step_real(kind, momentum):
 # c. through optim.Arena
 # ------------------------------------------------------------------------------------------------
 def test_arena_segments_padding_and_per_variable_hyper_parameters():
-    _C, rt = _lib()
+    _C, rt = lib()
     from pnp_b200 import optim
     gen = torch.Generator().manual_seed(3)
     vs = [(torch.randint(-16, 17, (s,), generator=gen).float() * 0.25).to(DEV) for s in ARENA_SIZES]
@@ -238,7 +221,7 @@ def test_arena_segments_padding_and_per_variable_hyper_parameters():
 def test_adam_graph_reads_the_advanced_lr():
     """[pnp_adam_advance, pnp_adam_step] captured once and replayed: after each replay the state equals the Python advance
     bit for bit and theta / m / v equal the reference step with that state's lr_t, within TAU"""
-    _C, rt = _lib()
+    _C, rt = lib()
     c = real_case("adam", 0.0, seed=29, n=8 * 1024, nseg=5)
     c["state"] = [1.0, 1.0, 1e-3, 0.0]
     d = dev(c)
@@ -280,11 +263,11 @@ REJECT = [(kind, what, change) for kind in ("adam", "rmsprop", "momentum") for w
 
 @pytest.mark.parametrize("kind,what,change", REJECT, ids=["%s_%s" % r[:2] for r in REJECT])
 def test_rejected_calls_leave_buffers_untouched(kind, what, change):
-    _C, rt = _lib()
+    _C, rt = lib()
     key = next(iter(change))
     c = O.dyadic_case(kind, 2048, 2, 1.0, seed=5)
     d = dev(c)
-    before = {k: d[k].clone() for k in O.OUTPUTS[kind]}
+    before = snapshot({k: d[k] for k in O.OUTPUTS[kind]})
     lr_t, state_t = scalars(kind, c)
     if key == "scalar":
         lr_t, state_t = None, None
@@ -294,9 +277,7 @@ def test_rejected_calls_leave_buffers_untouched(kind, what, change):
     rc = launch(_C, rt, kind, d, lr_t, state_t, checked=False)
     torch.cuda.synchronize()
     assert rc == BAD_ARG, "%s %s: returned %d" % (kind, what, rc)
-    for k, b in before.items():
-        if d[k] is not None:
-            assert torch.equal(d[k], b), "%s %s: %s changed" % (kind, what, k)
+    assert_untouched("%s %s" % (kind, what), kind, d, before)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -306,9 +287,5 @@ def test_rejected_calls_leave_buffers_untouched(kind, what, change):
 def test_exact_cases_under_pdl():
     """programmatic dependent launch lets each kernel start before its predecessor ends: the step must still see the advanced
     state and the previous step's outputs"""
-    env = dict(os.environ, PNP_PDL="1")
-    code = ("import sys; sys.path.insert(0, %r); from tests import test_optim_exact_gpu as T; "
-            "[T.test_step_exact(c) for c in T.EXACT_CASES if '2p24' not in c[0]]; T.test_adam_advance_matches_double(); "
-            "T.test_adam_graph_reads_the_advanced_lr(); print('pdl ok')" % ROOT)
-    r = subprocess.run([sys.executable, "-c", code], env=env, cwd=ROOT, capture_output=True, text=True, timeout=280)
-    assert r.returncode == 0 and "pdl ok" in r.stdout, r.stdout[-2000:] + r.stderr[-4000:]
+    passed, _ = rerun({"PNP_PDL": "1"}, __file__, "(step_exact and not 2p24) or adam_advance_matches_double or adam_graph_reads")
+    assert passed == len([c for c in EXACT_CASES if "2p24" not in c[0]]) + 2, passed

@@ -26,17 +26,17 @@ import numpy as np
 import pytest
 import torch
 
-from tests.test_tf_semantics_opencv_cpu import _have_cv2, const, node, placeholder, _protos
+from tests.opencv_graphdef import const, have_cv2, node, placeholder, protos
 
 pytest.importorskip("tensorboard")
-pytestmark = pytest.mark.skipif(not _have_cv2(), reason="OpenCV with the dnn module is not importable")
+pytestmark = pytest.mark.skipif(not have_cv2(), reason="OpenCV with the dnn module is not importable")
 HERE = os.path.dirname(os.path.abspath(__file__))
 REF = json.load(open(os.path.join(HERE, "golden", "reference_graph_trace.json")))
 B = 2
 
 
 def _run_opencv(d, name, nodes, x):
-    graph_pb2 = _protos()[0]
+    graph_pb2 = protos()[0]
     g = graph_pb2.GraphDef()
     g.node.extend(nodes)
     open(os.path.join(d, name + ".pb"), "wb").write(g.SerializeToString())
@@ -158,11 +158,11 @@ SEG_STATS = {"conv": 27, "atrous": 4, "bn": 30, "skip": 14, "pad_skip": 5, "pool
 @pytest.mark.timeout(1800)
 def test_reference_segmenter_graph_in_opencv_equals_the_oracle(tmp_path):
     from oracle.pnp_graphs import OracleSegmenter, init_numpy_params, synthetic_images
-    from tests.test_parity_configs_gpu import _bn_noise
+    from tests.models import bn_noise
     events = REF["source_segmenter"]["events"]
     ws, bns = OracleSegmenter.layout()
     P = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(P, bns, 6)
+    bn_noise(P, bns, 6)
     x = synthetic_images(B, 1234)
     t0 = time.time()
     c9, logits = run_stream_in_opencv(events, P, x.numpy(), str(tmp_path), SEG_STATS)
@@ -180,7 +180,7 @@ def test_reference_adversarial_segmenter_streams_in_opencv_equal_the_oracle(tmp_
     scopes adapt_*); create_second_half (group_7..output, AUTO_REUSE) is called first on the CT features, then on the MR features.
     Each stream's chain of traced layers, with the oracle's GAN-graph parameters, through OpenCV vs OracleAdversarial.segment."""
     from oracle.pnp_graphs import OracleAdversarial, init_numpy_params, synthetic_images
-    from tests.test_parity_configs_gpu import _bn_noise
+    from tests.models import bn_noise
     ev = REF["events"]
     zipn = [e for e in ev if e["section"] == "create_zip_network#1"]
     starts = [i for i, e in enumerate(zipn) if e.get("input_src")]
@@ -192,7 +192,7 @@ def test_reference_adversarial_segmenter_streams_in_opencv_equal_the_oracle(tmp_
     assert back[0]["w"] == "group_7/Variable" and back[-1]["w"] == "output/Variable"
     ws, bns = OracleAdversarial.layout()
     P = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(P, bns, 6)
+    bn_noise(P, bns, 6)
     x = synthetic_images(B, 1234) if stream == "mr" else synthetic_images(B, 4321, 0.3, 0.8)
     c9, logits = run_stream_in_opencv(front + back, P, x.numpy(), str(tmp_path), SEG_STATS)
     oracle = OracleAdversarial(P, B, lambda_mask_loss=0.3, dis_sub_iter=1, gen_sub_iter=1)
@@ -205,17 +205,17 @@ def test_committed_opencv_vectors_match_the_oracle():
     """the fixture the GPU tests compare the CUDA path with (tests/golden/opencv_reference_graph_vectors.npz) -- read back through the
     very helper the GPU tests use and held against the oracle here, so a fixture / indexing mistake cannot hide behind a GPU tolerance"""
     from oracle.pnp_graphs import OracleSegmenter, OracleAdversarial, init_numpy_params, synthetic_images
-    from tests.test_parity_configs_gpu import _bn_noise
+    from tests.models import bn_noise
     from tests.util import compare_with_opencv_vectors
     ws, bns = OracleSegmenter.layout()
     P = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(P, bns, 6)
+    bn_noise(P, bns, 6)
     with torch.no_grad():
         lg = OracleSegmenter(P, B).forward(synthetic_images(B, 1234), 1.0, False)["logits"]
     err, agree = compare_with_opencv_vectors("segmenter", lg, 2e-5, 0.99995)
     ws, bns = OracleAdversarial.layout()
     P = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(P, bns, 6)
+    bn_noise(P, bns, 6)
     with torch.no_grad():
         lg = OracleAdversarial(P, B, lambda_mask_loss=0.3, dis_sub_iter=1, gen_sub_iter=1).segment(
             synthetic_images(B, 4321, 0.3, 0.8), "ct", 1.0, False)["logits"]

@@ -16,8 +16,6 @@ e. PNP_TAIL5 (read once per process) = 0, 1, 2 re-runs the 5x5 tail cases in a p
 The C-ABI is called directly (_C.call / ptr / ConvGeom / DropCfg) on the runtime's stream; the fp64 references run on the device."""
 import ctypes
 import os
-import subprocess
-import sys
 import time
 
 import pytest
@@ -26,13 +24,10 @@ import torch
 from oracle import bf16_split as S
 from oracle import simt_exact as E
 from oracle.simt_exact import TailGeom
-from tests.test_tc_split_exact_gpu import drop_cfg, drop_mask, same_pad
+from tests.cabi import BAD_ARG, DEV, cpu_gen, drop_cfg, drop_mask, ints, lib, rerun, same_pad
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEV = "cuda"
 EXACT = 2.0 ** 24
-BAD_ARG = 100001
 
 
 def conv(B, H, W, Cin, Cout, kh, kw=None, s=1, d=1, pad="SAME"):
@@ -142,12 +137,6 @@ def int_launches():
 # ------------------------------------------------------------------------------------------------
 # C-ABI plumbing
 # ------------------------------------------------------------------------------------------------
-def _lib():
-    import pnp_b200  # noqa: F401
-    from pnp_b200 import _C, runtime as rt
-    return _C, rt
-
-
 def _fwd(_C, rt, x, w, y, g, drop=None, acc=0):
     _C.call("pnp_conv2d_fwd", _C.ptr(x), _C.ptr(w), _C.ptr(y), ctypes.byref(_C.ConvGeom(*[int(v) for v in g])),
             None if drop is None else ctypes.byref(drop), acc, rt.stream())
@@ -176,16 +165,12 @@ def _nan(*shape):
     return torch.full(shape, float("nan"), device=DEV)
 
 
-def _ints(shape, gen, dev=DEV):
-    return torch.randint(-4, 5, shape, generator=gen).float().to(dev)
-
-
 def _operands(g, seed, integer, dev=DEV):
     """fp32 x [B,H,W,Cin], w HWIO, dy [B,Ho,Wo,Cout] (on `dev`)"""
     gen = torch.Generator().manual_seed(seed)
     shapes = ((g.B, g.H, g.W, g.Cin), (g.kh, g.kw, g.Cin, g.Cout), (g.B, g.Ho, g.Wo, g.Cout))
     if integer:
-        return tuple(_ints(s, gen).to(dev) for s in shapes)
+        return tuple(ints(s, -4, 4, gen).to(dev) for s in shapes)
     x, w, dy = (torch.randn(s, generator=gen) for s in shapes)
     return x.to(dev), (w * 0.05).to(dev), dy.to(dev)
 
@@ -195,7 +180,7 @@ def _tail_operands(t, seed, integer, dev=DEV):
     gen = torch.Generator().manual_seed(seed)
     shapes = ((t.B, t.a, t.b, t.G * t.r * t.r), (t.kh, t.kw, t.G, t.Cout), (t.B, t.a * t.r, t.b * t.r, t.Cout))
     if integer:
-        return tuple(_ints(s, gen).to(dev) for s in shapes)
+        return tuple(ints(s, -4, 4, gen).to(dev) for s in shapes)
     X, w, dy = (torch.randn(s, generator=gen) for s in shapes)
     return X.to(dev), (w * 0.05).to(dev), dy.to(dev)
 
@@ -247,21 +232,21 @@ def _ids(cases):
 @pytest.mark.parametrize("case", FWD, ids=_ids(FWD))
 def test_fwd_exact(case):
     """plain, accumulating into a non-zero y, and (flagged cases) with dropout: mask * fp32(exact) at every element"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, g, flags = case
     x, w, _ = _operands(g, 11, True)
     ref, cond = S.fwd_bilinear(_d(x), _d(w), g), S.fwd_bilinear(_d(x).abs(), _d(w).abs(), g)
     y = _nan(g.B, g.Ho, g.Wo, g.Cout)
     _fwd(_C, rt, x, w, y, g)
     _exact(tag, y, ref, cond)
-    y0 = _ints((g.B, g.Ho, g.Wo, g.Cout), torch.Generator().manual_seed(12))
+    y0 = ints((g.B, g.Ho, g.Wo, g.Cout), -4, 4, cpu_gen(12)).to(DEV)
     y = y0.clone()
     _fwd(_C, rt, x, w, y, g, acc=1)
     _exact(tag + " acc", y, _d(y0) + ref, cond + _d(y0).abs())
     keep = _drop_keep(flags)
     if keep:
         cfg, seed_t = drop_cfg(_C, keep, stream_id=5)
-        mask = drop_mask(_C, rt, cfg, y.shape)
+        mask = drop_mask(cfg, y.shape)
         y = _nan(*y.shape)
         _fwd(_C, rt, x, w, y, g, drop=cfg)
         torch.cuda.synchronize()
@@ -274,7 +259,7 @@ def test_fwd_exact(case):
 @pytest.mark.parametrize("case", DGRAD, ids=_ids(DGRAD))
 def test_dgrad_exact(case):
     """dx = conv^T(dy, w) with w transposed by pnp_weight_transpose, plain and accumulating into a non-zero dx"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, g, _ = case
     _, w, dy = _operands(g, 21, True)
     wT = _transpose(_C, rt, w)
@@ -282,7 +267,7 @@ def test_dgrad_exact(case):
     dx = _nan(g.B, g.H, g.W, g.Cin)
     _dgrad(_C, rt, dy, wT, dx, g)
     _exact(tag, dx, ref, cond)
-    dx0 = _ints(dx.shape, torch.Generator().manual_seed(22))
+    dx0 = ints(dx.shape, -4, 4, cpu_gen(22)).to(DEV)
     dx = dx0.clone()
     _dgrad(_C, rt, dy, wT, dx, g, acc=1)
     _exact(tag + " acc", dx, _d(dx0) + ref, cond + _d(dx0).abs())
@@ -291,11 +276,11 @@ def test_dgrad_exact(case):
 @pytest.mark.parametrize("case", WGRAD, ids=_ids(WGRAD))
 def test_wgrad_exact(case):
     """dw += x (*) dy into a non-zero dw (the launcher always accumulates)"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, g, _ = case
     x, _, dy = _operands(g, 31, True)
     ref, cond = S.wgrad_bilinear(_d(x), _d(dy), g), S.wgrad_bilinear(_d(x).abs(), _d(dy).abs(), g)
-    dw0 = _ints((g.kh, g.kw, g.Cin, g.Cout), torch.Generator().manual_seed(32))
+    dw0 = ints((g.kh, g.kw, g.Cin, g.Cout), -4, 4, cpu_gen(32)).to(DEV)
     dw = dw0.clone()
     _wgrad(_C, rt, x, dy, dw, g)
     print("  %s: %s" % (tag, E.simt_instance("wgrad", g)))
@@ -304,7 +289,7 @@ def test_wgrad_exact(case):
 
 @pytest.mark.parametrize("taps,cin,cout", TRANSPOSE)
 def test_weight_transpose_exact(taps, cin, cout):
-    _C, rt = _lib()
+    _C, rt = lib()
     w = torch.randn(taps, 1, cin, cout, generator=torch.Generator().manual_seed(taps + cin)).to(DEV)
     wT = _transpose(_C, rt, w)
     torch.cuda.synchronize()
@@ -329,7 +314,7 @@ def _three_kernel_bwd(_C, rt, dy, w, t):
 def test_tail_exact(case):
     """pnp_ps_mirror_conv_fwd / _bwd against the fp64 composition conv(mirror_pad(PS(X))) and its autograd; the backward also
     equals the three-kernel route bit for bit where that route runs (square kernel, 2p <= H, W)"""
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, t, _ = case
     X, w, dy = _tail_operands(t, 41, True)
     H, W = t.a * t.r, t.b * t.r
@@ -359,7 +344,7 @@ def _real_cases(cases):
 
 @pytest.mark.parametrize("case", _real_cases(FWD), ids=_ids(_real_cases(FWD)))
 def test_fwd_real(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, g, _ = case
     x, w, _ = _operands(g, 51, False)
     y = _nan(g.B, g.Ho, g.Wo, g.Cout)
@@ -370,7 +355,7 @@ def test_fwd_real(case):
 
 @pytest.mark.parametrize("case", _real_cases(DGRAD), ids=_ids(_real_cases(DGRAD)))
 def test_dgrad_real(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, g, _ = case
     _, w, dy = _operands(g, 52, False)
     dx = _nan(g.B, g.H, g.W, g.Cin)
@@ -381,7 +366,7 @@ def test_dgrad_real(case):
 
 @pytest.mark.parametrize("case", _real_cases(WGRAD), ids=_ids(_real_cases(WGRAD)))
 def test_wgrad_real(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, g, _ = case
     x, _, dy = _operands(g, 53, False)
     dw0 = (torch.randn(g.kh, g.kw, g.Cin, g.Cout, generator=torch.Generator().manual_seed(54)) * 0.01).to(DEV)
@@ -393,7 +378,7 @@ def test_wgrad_real(case):
 
 @pytest.mark.parametrize("case", _real_cases(TAIL), ids=_ids(_real_cases(TAIL)))
 def test_tail_real(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     tag, t, _ = case
     X, w, dy = _tail_operands(t, 55, False)
     y = _nan(t.B, t.a * t.r, t.b * t.r, t.Cout)
@@ -414,7 +399,7 @@ def test_launched_kernels_match_restatement():
     """one launch per entry of int_launches() under torch.profiler; the SIMT kernel each one ran, in launch order, is
     simt_instance() of its geometry (the operands are zero: only the dispatch matters here)"""
     from torch.profiler import ProfilerActivity, profile
-    _C, rt = _lib()
+    _C, rt = lib()
     plan = int_launches()
     want = [E.simt_instance(l, g, drop, acc)[0] for l, g, drop, acc in plan]
     cfg, seed_t = drop_cfg(_C, 0.5, stream_id=9)
@@ -483,7 +468,7 @@ DECLINE = [
 
 @pytest.mark.parametrize("case", DECLINE, ids=_ids(DECLINE))
 def test_declined_launches_leave_output_untouched(case):
-    _C, rt = _lib()
+    _C, rt = lib()
     _, launcher, g, null, code = case
     src = torch.zeros(4096, device=DEV)
     wt = torch.zeros(4096, device=DEV)
@@ -516,12 +501,7 @@ def test_declined_launches_leave_output_untouched(case):
 def test_tail5_switch(mode):
     """PNP_TAIL5 bit 0 = register-tiled 5x5 forward, bit 1 = register-tiled 5x5 backward; every 5x5 tail case, integer and
     real, through the other kernel of each pair"""
-    env = dict(os.environ)
-    env["PNP_TAIL5"] = mode
-    t0 = time.time()
-    p = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-s", "-p", "no:cacheprovider", os.path.abspath(__file__),
-                        "-k", "(tail_exact or tail_real) and k5_"], cwd=ROOT, env=env, capture_output=True, text=True, timeout=280)
-    lines = p.stdout.splitlines()
+    passed, lines = rerun({"PNP_TAIL5": mode}, __file__, "(tail_exact or tail_real) and k5_", flags=("-s",))
     print("\n".join(l for l in lines if "RATIO" in l or "PNP_TAIL5" in l))
-    print("  PNP_TAIL5=%s: %s (wall %.1f s)" % (mode, lines[-1] if lines else "", time.time() - t0))
-    assert p.returncode == 0, "\n".join(lines[-25:])
+    k5 = [c for c in TAIL if c[0].startswith("k5_")]
+    assert passed == len(k5) + len(_real_cases(k5)), passed

@@ -218,7 +218,7 @@ def test_test_eval_surface_metrics_both_trainers(tmp_path, capsys):
     from pnp_b200.lib import write_nii
     from pnp_b200.train_gan import configure
     from oracle.pnp_graphs import OracleAdversarial, OracleSegmenter, init_numpy_params
-    from tests.test_parity_configs_gpu import _bn_noise
+    from tests.models import bn_noise
     rt.set_conv_backend("auto")
     B = 2
     rng = np.random.RandomState(33)
@@ -232,7 +232,7 @@ def test_test_eval_surface_metrics_both_trainers(tmp_path, capsys):
 
     ws, bns = OracleAdversarial.layout()
     P = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(P, bns, 6)
+    bn_noise(P, bns, 6)
     ck, nc, tc = configure("train-gan")
     net = adv.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=ck, network_config=nc)
     rt.load_state_dict(P)
@@ -260,7 +260,7 @@ def test_test_eval_surface_metrics_both_trainers(tmp_path, capsys):
 
     ws, bns = OracleSegmenter.layout()
     Ps = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(Ps, bns, 6)
+    bn_noise(Ps, bns, 6)
     snet = seg.Full_DRN(channels=3, n_class=5, batch_size=B,
                         cost_kwargs={"cross_flag": True, "miu_cross": 1.0, "dice_flag": True, "miu_dice": 1.0})
     rt.load_state_dict(Ps)

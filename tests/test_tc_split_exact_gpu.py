@@ -13,19 +13,15 @@ The C-ABI is called directly (_C.call / ptr / ConvGeom / TcEpilogue) on the runt
 device too.  Each conv test prints its worst ratio |got - ref| / sum|a||b| next to TAU."""
 import ctypes
 import os
-import subprocess
-import sys
-import time
 
 import pytest
 import torch
 
 from oracle import bf16_split as S
-from oracle import philox
+from tests.cabi import (DEV, assert_planes, drop_cfg, drop_mask, empty_planes, expected_ksplit, last_config, lib, rerun, same_pad,
+                        sm_count, split_dev, split_w_dev)
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEV = "cuda"
 U32 = 2.0 ** -23      # one fp32 ulp, relative
 
 # (id, B, H, W, Cin, Cout, k, stride, dil, padding, what it reaches; flags)
@@ -57,12 +53,6 @@ CASES = [
 CASE_IDS = [c[0] for c in CASES]
 
 
-def same_pad(n, k, s, d=1):
-    out = -(-n // s)
-    total = max((out - 1) * s + (k - 1) * d + 1 - n, 0)
-    return total // 2
-
-
 def geom_of(case):
     """-> oracle Geom (SYMMETRIC: H, W of the already mirror-padded input, VALID conv)"""
     _, B, H, W, Cin, Cout, k, s, d, pad, _ = case
@@ -72,52 +62,6 @@ def geom_of(case):
         Ho, Wo = (Hp - (k - 1) * d - 1) // s + 1, (Wp - (k - 1) * d - 1) // s + 1
         return S.Geom(B, Hp, Wp, Cin, Ho, Wo, Cout, k, k, s, d, 0, 0)
     return S.Geom(B, H, W, Cin, -(-H // s), -(-W // s), Cout, k, k, s, d, same_pad(H, k, s, d), same_pad(W, k, s, d))
-
-
-def _choose_tile(U, V, B):
-    """pixel tile (tw, th, tn) of 128 output pixels over a U x V grid (conv_tc.cu choose_tile, exact = 0)"""
-    if V >= 128:
-        return 128, 1, 1
-    tw, th = V, min(128 // V, U)
-    tn = max(128 // (tw * th), 1) if th == U else 1
-    return tw, th, min(tn, B)
-
-
-def _k_block(n_cols, K):
-    bk = 64 if K % 64 == 0 else (32 if K % 32 == 0 else 16)
-    if bk == 64 and n_cols in (128, 64) and os.environ.get("PNP_TC_BK%d" % n_cols, "64").strip() == "32":
-        bk = 32
-    return bk
-
-
-def expected_ksplit(launcher, g, sms):
-    """split-K factor the forward / data-gradient launcher picks for geometry g (no fused epilogue) on a device with `sms`
-    SMs, restating the rule of conv_tc.cu run_tc: split when the layer has at most half as many tiles as SMs and at least 8
-    k-blocks in its shallowest phase, by min(sms / tiles, k-blocks / 4, 32)"""
-    cdiv = lambda a, b: -(-a // b)  # noqa: E731
-    if launcher == "fwd":
-        N, K = g.Cout, g.Cin
-        phases = [(g.Ho, g.Wo, g.kh * g.kw)]
-    else:
-        N, K, s = g.Cin, g.Cout, g.stride
-        phases = []
-        for py in range(s):
-            for px in range(s):
-                Up, Vp = (g.H - py + s - 1) // s, (g.W - px + s - 1) // s
-                if Up <= 0 or Vp <= 0:
-                    continue
-                ty = sum(1 for k in range(g.kh) if (py + g.pad_t - k * g.dil) % s == 0)
-                tx = sum(1 for k in range(g.kw) if (px + g.pad_l - k * g.dil) % s == 0)
-                phases.append((Up, Vp, ty * tx))
-    U, V = max(p[0] for p in phases), max(p[1] for p in phases)
-    tw, th, tn = _choose_tile(U, V, g.B)
-    n_cols = 128 if N % 128 == 0 else (64 if N % 64 == 0 else (32 if N % 32 == 0 else 16))
-    kchunks = K // _k_block(n_cols, K)
-    tiles = sum(cdiv(Vp, tw) * cdiv(Up, th) for Up, Vp, _ in phases) * cdiv(g.B, tn) * (N // n_cols)
-    min_kb = min(t for _, _, t in phases) * kchunks
-    if tiles * 2 > sms or min_kb < 8:
-        return 1
-    return max(1, min(sms // tiles, min_kb // 4, 32))
 
 
 def operands(g, seed):
@@ -132,61 +76,8 @@ def operands(g, seed):
 # ------------------------------------------------------------------------------------------------
 # C-ABI plumbing
 # ------------------------------------------------------------------------------------------------
-def _lib():
-    import pnp_b200  # noqa: F401
-    from pnp_b200 import _C, runtime as rt
-    if not rt.tc_available():
-        pytest.fail("wgmma path unavailable on this device -- it must be the one that runs on H100")
-    return _C, rt
-
-
 def _cgeom(_C, g):
     return _C.ConvGeom(*[int(v) for v in g])
-
-
-def _planes(shape, nterms):
-    hi = torch.empty(shape, dtype=torch.bfloat16, device=DEV)
-    return hi, (torch.empty(shape, dtype=torch.bfloat16, device=DEV) if nterms == 3 else None)
-
-
-def split_dev(_C, rt, x, nterms):
-    hi, lo = _planes(x.shape, nterms)
-    _C.call("pnp_split_bf16", _C.ptr(x), _C.ptr(hi), _C.ptr(lo), x.numel(), rt.stream())
-    return hi, lo
-
-
-def split_w_dev(_C, rt, w, for_dgrad, nterms, cin_pad=0):
-    kh, kw, cin, cout = w.shape
-    hi, lo = _planes((kh * kw * max(cin, cin_pad) * cout,), nterms)
-    _C.call("pnp_split_weight_bf16", _C.ptr(w), _C.ptr(hi), _C.ptr(lo), kh, kw, cin, cout, 1 if for_dgrad else 0, cin_pad,
-            rt.stream())
-    return hi, lo
-
-
-def sm_count():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-
-
-def last_config(_C):
-    n_, k_, s_ = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_int(0)
-    _C.lib.pnp_tc_last_config(ctypes.byref(n_), ctypes.byref(k_), ctypes.byref(s_))
-    return n_.value, k_.value, s_.value
-
-
-def drop_cfg(_C, keep, stream_id=11, seed=0x1234_5678_9ABC):
-    seed_t = torch.tensor([seed], dtype=torch.int64, device=DEV)
-    cfg = _C.DropCfg(seed_t.data_ptr(), stream_id, keep)
-    cfg.seed_value = seed
-    return cfg, seed_t
-
-
-def drop_mask(_C, rt, cfg, shape):
-    """the multipliers of (seed, stream, keep) from the independent Philox4x32-10 reference (oracle/philox.py)"""
-    n = 1
-    for s in shape:
-        n *= int(s)
-    m = philox.dropout_mult(cfg.seed_value, cfg.stream, cfg.keep, n)
-    return torch.from_numpy(m).reshape(tuple(shape)).to(DEV)
 
 
 def _f64(t):
@@ -219,16 +110,9 @@ def edge_values():
     return torch.tensor([p - (1 << 32) if p >= (1 << 31) else p for p in pats], dtype=torch.int32).view(torch.float32)
 
 
-def _assert_planes(tag, hi, lo, fp32):
-    rh, rl = S.split(fp32.cpu())
-    assert S.planes_equal(hi.cpu().reshape(rh.shape), rh), "%s: hi plane is not rn_bf16(x)" % tag
-    if lo is not None:
-        assert S.planes_equal(lo.cpu().reshape(rl.shape), rl), "%s: lo plane is not rn_bf16(x - hi)" % tag
-
-
 @pytest.mark.parametrize("n", [1, 2, 3, 5, 7, 27, 1_000_003])
 def test_split_bf16_planes_are_exact(n):
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     gen = torch.Generator().manual_seed(n)
     x = torch.randn(n, generator=gen) * torch.exp2(torch.randint(-140, 120, (n,), generator=gen).float())
     e = edge_values()
@@ -237,24 +121,24 @@ def test_split_bf16_planes_are_exact(n):
     for nterms in (3, 1):
         hi, lo = split_dev(_C, rt, x, nterms)
         torch.cuda.synchronize()
-        _assert_planes("pnp_split_bf16 n=%d nterms=%d" % (n, nterms), hi, lo, x)
+        assert_planes("pnp_split_bf16 n=%d nterms=%d" % (n, nterms), hi, lo, x)
 
 
 def test_split_bf16_pad_planes_are_exact():
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     for rows, C, Cpad in ((37, 32, 64), (5, 4, 16), (300, 48, 64), (9, 64, 64)):
         x = (torch.randn(rows, C) * 3).to(DEV)
         hi = torch.full((rows, Cpad), 1.0, dtype=torch.bfloat16, device=DEV)
         lo = torch.full((rows, Cpad), 1.0, dtype=torch.bfloat16, device=DEV)
         _C.call("pnp_split_bf16_pad", _C.ptr(x), _C.ptr(hi), _C.ptr(lo), rows, C, Cpad, rt.stream())
         torch.cuda.synchronize()
-        _assert_planes("pnp_split_bf16_pad", hi[:, :C].contiguous(), lo[:, :C].contiguous(), x)
+        assert_planes("pnp_split_bf16_pad", hi[:, :C].contiguous(), lo[:, :C].contiguous(), x)
         assert int(S.bits(hi[:, C:]).abs().sum()) == 0 and int(S.bits(lo[:, C:]).abs().sum()) == 0, "padding channels not zero"
 
 
 @pytest.mark.parametrize("kh,Cin,Cout,cin_pad", [(3, 64, 128, 0), (5, 32, 64, 64), (1, 16, 16, 0), (3, 48, 40, 64), (3, 5, 33, 0)])
 def test_split_weight_planes_are_exact(kh, Cin, Cout, cin_pad):
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     w = torch.randn(kh, kh, Cin, Cout) * 0.05
     w.view(-1)[:27] = edge_values()[:27]
     w = w.to(DEV)
@@ -263,11 +147,11 @@ def test_split_weight_planes_are_exact(kh, Cin, Cout, cin_pad):
     cp = max(Cin, cin_pad)
     wf = torch.zeros(kh * kh, Cout, cp)
     wf[:, :, :Cin] = w.cpu().reshape(kh * kh, Cin, Cout).permute(0, 2, 1)
-    _assert_planes("split_weight fwd layout", hi, lo, wf.reshape(-1))
+    assert_planes("pnp_split_weight_bf16 fwd layout", hi, lo, wf.reshape(-1))
     if cin_pad <= Cin:
         hi, lo = split_w_dev(_C, rt, w, True, 3)
         torch.cuda.synchronize()
-        _assert_planes("split_weight dgrad layout", hi, lo, w.cpu().reshape(-1))
+        assert_planes("pnp_split_weight_bf16 dgrad layout", hi, lo, w.cpu().reshape(-1))
 
 
 def _bn_inputs(M, C, seed):
@@ -280,23 +164,23 @@ def _bn_inputs(M, C, seed):
 
 @pytest.mark.parametrize("act", [0, 1, 2])
 def test_bn_act_apply_planes(act):
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     M, C = 1000, 96
     z, scale, shift, _, _, skip_src = _bn_inputs(M, C, 5 + act)
     skip = skip_src[:, :32].contiguous()
     for sk, Cs, off in ((None, 0, 0), (skip, 32, 40)):
         y = torch.empty(M, C, device=DEV)
-        hi, lo = _planes((M, C), 3)
+        hi, lo = empty_planes((M, C), 3)
         _C.call("pnp_bn_act_apply", _C.ptr(z), _C.ptr(scale), _C.ptr(shift), _C.ptr(sk), Cs, off, act, _C.ptr(y), _C.ptr(hi),
                 _C.ptr(lo), M, C, rt.stream())
         torch.cuda.synchronize()
-        _assert_planes("pnp_bn_act_apply act=%d skip=%s" % (act, sk is not None), hi, lo, y)
+        assert_planes("pnp_bn_act_apply act=%d skip=%s" % (act, sk is not None), hi, lo, y)
 
 
 @pytest.mark.parametrize("training", [1, 0])
 @pytest.mark.parametrize("act", [0, 1, 2])
 def test_bn_apply_fused_planes(training, act):
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     M, C = 2048, 128
     z, gamma, beta, mm, mv, skip_src = _bn_inputs(M, C, 17 + act)
     zs = z.double()
@@ -305,13 +189,13 @@ def test_bn_apply_fused_planes(training, act):
     outs = []
     for with_y in (True, False):
         y = torch.empty(M, C, device=DEV) if with_y else None
-        hi, lo = _planes((M, C), 3)
+        hi, lo = empty_planes((M, C), 3)
         mm_, mv_ = mm.clone(), mv.clone()
         _C.call("pnp_bn_apply_fused", _C.ptr(z), _C.ptr(s1), _C.ptr(s2), M, C, _C.ptr(gamma), _C.ptr(beta), _C.ptr(mm_), _C.ptr(mv_),
                 training, _C.ptr(skip), 64, 32, act, _C.ptr(y), _C.ptr(hi), _C.ptr(lo), None, None, rt.stream())
         torch.cuda.synchronize()
         if with_y:
-            _assert_planes("pnp_bn_apply_fused train=%d act=%d" % (training, act), hi, lo, y)
+            assert_planes("pnp_bn_apply_fused train=%d act=%d" % (training, act), hi, lo, y)
         outs.append((hi, lo))
     assert torch.equal(S.bits(outs[0][0]), S.bits(outs[1][0])) and torch.equal(S.bits(outs[0][1]), S.bits(outs[1][1])), \
         "planes-only launch wrote different planes"
@@ -320,7 +204,7 @@ def test_bn_apply_fused_planes(training, act):
 @pytest.mark.parametrize("keep", [1.0, 0.75])
 @pytest.mark.parametrize("training", [1, 0])
 def test_bn_bwd_apply_planes(keep, training):
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     M, C = 3000, 64
     z, gamma, _, mean, var, g = _bn_inputs(M, C, 31)
     invstd = torch.rsqrt(var + 1e-3)
@@ -328,19 +212,19 @@ def test_bn_bwd_apply_planes(keep, training):
     dref = None if dcfg is None else ctypes.byref(dcfg)
     coef = (torch.randn(2 * C) * 0.1).to(DEV)
     dz = torch.empty(M, C, device=DEV)
-    hi, lo = _planes((M, C), 3)
+    hi, lo = empty_planes((M, C), 3)
     _C.call("pnp_bn_bwd_apply", _C.ptr(g), _C.ptr(z), _C.ptr(mean), _C.ptr(invstd), _C.ptr(gamma), _C.ptr(coef), training, dref,
             _C.ptr(dz), _C.ptr(hi), _C.ptr(lo), M, C, rt.stream())
     torch.cuda.synchronize()
-    _assert_planes("pnp_bn_bwd_apply", hi, lo, dz)
+    assert_planes("pnp_bn_bwd_apply", hi, lo, dz)
     gs = g.double()
     sg, sgx = gs.sum(0).contiguous(), (gs * ((z.double() - mean.double()) * invstd.double())).sum(0).contiguous()
     dz = torch.empty(M, C, device=DEV)
-    hi, lo = _planes((M, C), 3)
+    hi, lo = empty_planes((M, C), 3)
     _C.call("pnp_bn_bwd_apply_fused", _C.ptr(g), _C.ptr(z), _C.ptr(mean), _C.ptr(invstd), _C.ptr(gamma), _C.ptr(sg), _C.ptr(sgx), M, C,
             training, dref, None, None, _C.ptr(dz), _C.ptr(hi), _C.ptr(lo), rt.stream())
     torch.cuda.synchronize()
-    _assert_planes("pnp_bn_bwd_apply_fused", hi, lo, dz)
+    assert_planes("pnp_bn_bwd_apply_fused", hi, lo, dz)
     # direct: g recomputed from dy and the activation sign (from y, or from y's hi plane); planes-only == planes with fp32
     y = torch.randn(M, C).to(DEV)
     yhi, _ = split_dev(_C, rt, y, 1)
@@ -349,13 +233,13 @@ def test_bn_bwd_apply_planes(keep, training):
             outs = []
             for with_dz in (True, False):
                 dz = torch.empty(M, C, device=DEV) if with_dz else None
-                hi, lo = _planes((M, C), 3)
+                hi, lo = empty_planes((M, C), 3)
                 _C.call("pnp_bn_bwd_apply_direct", _C.ptr(g), _C.ptr(y if src == "y" else None), _C.ptr(yhi if src == "y_hi" else None),
                         act, _C.ptr(z), _C.ptr(mean), _C.ptr(invstd), _C.ptr(gamma), _C.ptr(sg), _C.ptr(sgx), M, C, training, dref,
                         None, None, _C.ptr(dz), _C.ptr(hi), _C.ptr(lo), rt.stream())
                 torch.cuda.synchronize()
                 if with_dz:
-                    _assert_planes("pnp_bn_bwd_apply_direct act=%d %s" % (act, src), hi, lo, dz)
+                    assert_planes("pnp_bn_bwd_apply_direct act=%d %s" % (act, src), hi, lo, dz)
                 outs.append((S.bits(hi), S.bits(lo)))
             assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1]), "planes-only dz planes differ"
 
@@ -422,7 +306,7 @@ def _xshape(g):
 @pytest.mark.parametrize("case", CASES, ids=CASE_IDS)
 def test_conv_split_exact(case, nterms):
     """fwd (+accumulate, dropout, BN sums), dgrad (+accumulate), wgrad (+accumulate) per element against the split reference"""
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     tag, flags = case[0], case[-1]
     P = Prepared(_C, rt, case, nterms)
     g = P.g
@@ -450,7 +334,7 @@ def test_conv_split_exact(case, nterms):
     # -- forward with dropout: mask (x) conv_split at every element, with the multiplier of pnp_dropout_apply
     if "drop" in flags:
         cfg, seed_t = drop_cfg(_C, 0.75)
-        mask = drop_mask(_C, rt, cfg, _yshape(g)).double()
+        mask = drop_mask(cfg, _yshape(g)).double()
         y = torch.full(_yshape(g), float("nan"), device=DEV)
         _fwd(_C, rt, P.xh, P.xl, P.wh, P.wl, y, g, nterms, drop=cfg)
         torch.cuda.synchronize()
@@ -508,7 +392,7 @@ EP_CASES = [c for c in CASES if "ep" in c[-1]]
 def test_conv_fused_epilogue_split_exact(case, act, nterms):
     """y = act(dropout(conv) * scale + shift + skip) against the fp64 epilogue of the split reference; its bf16 planes are
     split(y) bit for bit (tc1: hi only, y_lo = NULL), and a planes-only launch (y = NULL) writes the same planes"""
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     tag, flags = case[0], case[-1]
     P = Prepared(_C, rt, case, nterms)
     g = P.g
@@ -519,7 +403,7 @@ def test_conv_fused_epilogue_split_exact(case, act, nterms):
     skip = torch.randn(g.B, g.Ho, g.Wo, skip_c, generator=gen).to(DEV)
     cfg, seed_t = drop_cfg(_C, 0.75, stream_id=23) if "drop" in flags else (None, None)
     ref, cond = P.fwd_ref()
-    mask = drop_mask(_C, rt, cfg, _yshape(g)).double() if cfg is not None else torch.ones(_yshape(g), dtype=torch.float64, device=DEV)
+    mask = drop_mask(cfg, _yshape(g)).double() if cfg is not None else torch.ones(_yshape(g), dtype=torch.float64, device=DEV)
     sc, sh = scale.double(), shift.double()
     sk = torch.zeros(_yshape(g), dtype=torch.float64, device=DEV)
     sk[..., skip_off:skip_off + skip_c] = skip.double()
@@ -528,19 +412,19 @@ def test_conv_fused_epilogue_split_exact(case, act, nterms):
     out = pre if act == 0 else (pre.clamp_min(0) if act == 1 else torch.where(pre > 0, pre, 0.2 * pre))
     bound_cond = mask * cond * sc.abs()
     slack = 4 * U32 * (zs.abs() + sh.abs() + sk.abs())
-    planes = []
+    written = []
     for with_y in (True, False):
         y = torch.full(_yshape(g), float("nan"), device=DEV) if with_y else None
-        yh, yl = _planes(_yshape(g), nterms)
+        yh, yl = empty_planes(_yshape(g), nterms)
         ep = _C.TcEpilogue(_C.ptr(scale), _C.ptr(shift), _C.ptr(skip), skip_c, skip_off, act, _C.ptr(yh), _C.ptr(yl))
         _fwd(_C, rt, P.xh, P.xl, P.wh, P.wl, y, g, nterms, drop=cfg, ep=ep)
         torch.cuda.synchronize()
         assert last_config(_C)[2] == 1
         if with_y:
             _check("%s ep act=%d" % (tag, act), "fwd", nterms, y, out, bound_cond, slack=slack)
-            _assert_planes("%s epilogue planes" % tag, yh, yl, y)
-        planes.append([S.bits(p) for p in (yh, yl) if p is not None])
-    assert all(torch.equal(a, b) for a, b in zip(*planes)), "planes-only epilogue wrote different planes"
+            assert_planes("%s epilogue planes" % tag, yh, yl, y)
+        written.append([S.bits(p) for p in (yh, yl) if p is not None])
+    assert all(torch.equal(a, b) for a, b in zip(*written)), "planes-only epilogue wrote different planes"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -548,7 +432,7 @@ def test_conv_fused_epilogue_split_exact(case, act, nterms):
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("case", [CASES[3], CASES[1]], ids=[CASES[3][0], CASES[1][0]])
 def test_split_check_rejects_broken_launches(case):
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     tag = case[0]
     P = Prepared(_C, rt, case, 3)
     g = P.g
@@ -600,7 +484,7 @@ DECLINE = [
 
 @pytest.mark.parametrize("launcher,g", DECLINE, ids=["%s_%d" % (d[0], i) for i, d in enumerate(DECLINE)])
 def test_unsupported_shapes_are_declined_untouched(launcher, g):
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     xh = torch.zeros(g.B * g.H * g.W * g.Cin, dtype=torch.bfloat16, device=DEV)
     dh = torch.zeros(g.B * g.Ho * g.Wo * g.Cout, dtype=torch.bfloat16, device=DEV)
     wh = torch.zeros(g.kh * g.kw * g.Cin * g.Cout, dtype=torch.bfloat16, device=DEV)
@@ -620,7 +504,7 @@ def test_unsupported_shapes_are_declined_untouched(launcher, g):
 def test_accumulate_with_bn_sums_is_rejected():
     """batch statistics of an accumulating forward would be of the new contribution on one path and of old + new on the
     split-K path: the launcher refuses the combination"""
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     for case in (CASES[1], CASES[3]):            # split-K (on an H100) and single-pass forward
         g = geom_of(case)
         P = Prepared(_C, rt, case, 3)
@@ -638,7 +522,7 @@ def test_accumulate_with_bn_sums_is_rejected():
 # ------------------------------------------------------------------------------------------------
 def test_last_config_reports_k_block():
     """PNP_TC_BK128 / PNP_TC_BK64 = 32 select the <128,*,32> / <64,*,32> instantiations for 64-multiple reductions"""
-    _C, rt = _lib()
+    _C, rt = lib(require_tc=True)
     want = {128: int(os.environ.get("PNP_TC_BK128", "64")) == 32 and 32 or 64,
             64: int(os.environ.get("PNP_TC_BK64", "64")) == 32 and 32 or 64}
     for case, bn in ((CASES[3], 128), (CASES[12], 64)):
@@ -649,31 +533,29 @@ def test_last_config_reports_k_block():
         assert last_config(_C)[:2] == (bn, want[bn]), (case[0], last_config(_C))
 
 
-def _run(env_extra, kexpr):
-    env = dict(os.environ)
-    env.update(env_extra)
-    t0 = time.time()
-    p = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-s", "-p", "no:cacheprovider", os.path.abspath(__file__),
-                        "-k", kexpr], cwd=ROOT, env=env, capture_output=True, text=True, timeout=280)
-    lines = p.stdout.splitlines()
-    print("\n".join(l for l in lines if "RATIO" in l or "BN sums" in l))
-    print("  %s: %s (wall %.1f s)" % (env_extra, lines[-1] if lines else "", time.time() - t0))
-    assert p.returncode == 0, "\n".join(lines[-25:])
-
-
 # each switch re-runs only the cases whose kernels it changes: the K-block switches the 128- and 64-column tiles over 64-multiple
 # reductions (and the tile report); the taps-inner order and the rotation the multi-chunk reductions (rotation needs >= 16
 # k-blocks); programmatic dependent launch every kernel family once (plane producers, plain, split-K and phase convolutions,
-# the fused epilogue)
+# the fused epilogue).  The last entry is the number of tests each selection runs.
+def _n(cases, *names):
+    return sum(1 for c in cases if any(n in c[0] for n in names))
+
+
 SWITCHES = [
     ({"PNP_TC_BK128": "32", "PNP_TC_BK64": "32"},
-     "last_config or (conv_split_exact and (g10 or dil2 or 256x512 or 64_s2_256wide or 64_12x20 or wg_cin64))"),
-    ({"PNP_TC_ORDER": "1", "PNP_TC_ROT": "0"}, "conv_split_exact and (g10 or dil2 or k5s4 or 256x512 or wg_cin192)"),
-    ({"PNP_PDL": "1"}, "split_bf16 or bn_ or (conv_split_exact and (k5s4 or 256x512 or 16x32_k5s4)) or (epilogue and 64x32)"),
+     "last_config or (conv_split_exact and (g10 or dil2 or 256x512 or 64_s2_256wide or 64_12x20 or wg_cin64))",
+     1 + 2 * _n(CASES, "g10", "dil2", "256x512", "64_s2_256wide", "64_12x20", "wg_cin64")),
+    ({"PNP_TC_ORDER": "1", "PNP_TC_ROT": "0"}, "conv_split_exact and (g10 or dil2 or k5s4 or 256x512 or wg_cin192)",
+     2 * _n(CASES, "g10", "dil2", "k5s4", "256x512", "wg_cin192")),
+    ({"PNP_PDL": "1"}, "split_bf16 or bn_ or (conv_split_exact and (k5s4 or 256x512 or 16x32_k5s4)) or (epilogue and 64x32)",
+     # split_bf16: 7 sizes + the padded split; bn_: 3 + 6 + 4 plane tests and the accumulate-with-BN-sums rejection
+     8 + 14 + 2 * _n(CASES, "k5s4", "256x512") + 6 * _n(EP_CASES, "64x32")),
 ]
 
 
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize("env,kexpr", SWITCHES, ids=["bk32", "order1_rot0", "pdl"])
-def test_switch_variants(env, kexpr):
-    _run(env, kexpr)
+@pytest.mark.parametrize("env,kexpr,n", SWITCHES, ids=["bk32", "order1_rot0", "pdl"])
+def test_switch_variants(env, kexpr, n):
+    passed, lines = rerun(env, __file__, kexpr, flags=("-s",))
+    print("\n".join(l for l in lines if "RATIO" in l or "BN sums" in l))
+    assert passed == n, "%s: %d of %d tests passed" % (env, passed, n)

@@ -19,64 +19,11 @@ import sys
 import numpy as np
 import pytest
 
+from tests.opencv_graphdef import const, have_cv2, node, placeholder, protos
+
 pytest.importorskip("tensorboard")
 HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _have_cv2():
-    p = subprocess.run([sys.executable, "-c", "import cv2; print(hasattr(cv2.dnn, 'readNetFromTensorflow'))"], capture_output=True, text=True)
-    return p.returncode == 0 and p.stdout.strip() == "True"
-
-
-pytestmark = pytest.mark.skipif(not _have_cv2(), reason="OpenCV with the dnn module is not importable")
-
-
-# ---- GraphDef construction with the TF protos bundled in tensorboard -----------------------------------------------------------
-def _protos():
-    from tensorboard.compat.proto import graph_pb2, node_def_pb2, tensor_pb2, tensor_shape_pb2, types_pb2
-    return graph_pb2, node_def_pb2, tensor_pb2, tensor_shape_pb2, types_pb2
-
-
-def _shape(dims):
-    _, _, _, ts, _ = _protos()
-    return ts.TensorShapeProto(dim=[ts.TensorShapeProto.Dim(size=int(d)) for d in dims])
-
-
-def const(name, arr, integer=False):
-    _, nd, tp, _, ty = _protos()
-    arr = np.asarray(arr)
-    dt = ty.DT_INT32 if integer else ty.DT_FLOAT
-    n = nd.NodeDef(name=name, op="Const")
-    n.attr["dtype"].type = dt
-    n.attr["value"].tensor.CopyFrom(tp.TensorProto(dtype=dt, tensor_shape=_shape(arr.shape),
-                                                   tensor_content=arr.astype("<i4" if integer else "<f4").tobytes()))
-    return n
-
-
-def placeholder(name, shape):
-    _, nd, _, _, ty = _protos()
-    n = nd.NodeDef(name=name, op="Placeholder")
-    n.attr["dtype"].type = ty.DT_FLOAT
-    n.attr["shape"].shape.CopyFrom(_shape(shape))
-    return n
-
-
-def node(name, op, inputs, **attrs):
-    _, nd, _, _, ty = _protos()
-    n = nd.NodeDef(name=name, op=op, input=list(inputs))
-    n.attr["T"].type = ty.DT_FLOAT
-    for k, v in attrs.items():
-        if isinstance(v, bytes):
-            n.attr[k].s = v
-        elif isinstance(v, bool):
-            n.attr[k].b = v
-        elif isinstance(v, float):
-            n.attr[k].f = v
-        elif isinstance(v, int):
-            n.attr[k].i = v
-        else:
-            n.attr[k].list.i.extend(int(i) for i in v)
-    return n
+pytestmark = pytest.mark.skipif(not have_cv2(), reason="OpenCV with the dnn module is not importable")
 
 
 class Batch(object):
@@ -86,7 +33,7 @@ class Batch(object):
         self.d, self.cases = str(d), []
 
     def add(self, name, nodes, x, expected, tol):
-        graph_pb2 = _protos()[0]
+        graph_pb2 = protos()[0]
         g = graph_pb2.GraphDef()
         g.node.extend(nodes)
         open(os.path.join(self.d, name + ".pb"), "wb").write(g.SerializeToString())

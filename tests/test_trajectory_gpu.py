@@ -31,7 +31,7 @@ import pytest
 import torch
 
 from tests.util import l2_err
-from tests.test_parity_configs_gpu import adv_pair, seg_pair, loss_close, state_close
+from tests.models import adv_pair, seg_pair, loss_close, state_close
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"

@@ -12,7 +12,7 @@ import pytest
 import torch
 
 from tests.util import compare_with_opencv_vectors
-from tests.test_parity_configs_gpu import _bn_noise
+from tests.models import bn_noise
 
 pytestmark = pytest.mark.gpu
 B = 2
@@ -27,7 +27,7 @@ def test_segmenter_logits_match_the_opencv_executed_reference_graph(backend):
     try:
         ws, bns = OracleSegmenter.layout()
         P = init_numpy_params(ws, bns, 0, 0.05)
-        _bn_noise(P, bns, 6)
+        bn_noise(P, bns, 6)
         net = seg.Full_DRN(channels=3, n_class=5, batch_size=B,
                            cost_kwargs={"cross_flag": True, "miu_cross": 1.0, "dice_flag": True, "miu_dice": 1.0})
         rt.load_state_dict(P)
@@ -47,7 +47,7 @@ def test_adapted_ct_stream_logits_match_the_opencv_executed_reference_graph():
     rt.set_conv_backend("auto")
     ws, bns = OracleAdversarial.layout()
     P = init_numpy_params(ws, bns, 0, 0.05)
-    _bn_noise(P, bns, 6)
+    bn_noise(P, bns, 6)
     ck, nc, tc = configure("train-gan")
     net = adv.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=ck, network_config=nc)
     rt.load_state_dict(P)
