@@ -572,7 +572,8 @@ class Trainer(object):
     def _capture(self, fn, warmup):
         """Capture `fn()` (forward, backward, all-reduce, optimizer, clip: ~1 k kernel launches) into one CUDA graph.
         Dropout seeds, optimizer hyper-state and BN statistics live in device memory, so every replay is a genuinely new
-        training step.  Returns (graph, outputs) or (None, None) -- loudly -- if capture fails."""
+        training step.  Returns (graph, outputs, the moving statistics the step trains) or (None, None, []) -- loudly -- if
+        capture fails."""
         try:
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
@@ -586,20 +587,22 @@ class Trainer(object):
             # every replay would run on pre-capture weights.  Drop them so the captured step re-derives them from the live
             # arenas, and keep the variables' versions moving on every replay for eager code that runs later.
             self._invalidate_operand_caches()
+            # (the moving statistics the captured step trains include the critics', whose gamma / beta the G arena does not hold)
+            before = rt.moving_stat_versions()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 out = fn()
-            return g, out
+            return g, out, rt.moving_stats_bumped_since(before)
         except Exception as e:      # noqa: BLE001 -- any capture problem => eager path, loudly
             import warnings
             warnings.warn("CUDA-graph capture of the adversarial step failed (%s: %s); running eagerly" % (type(e).__name__, e))
             torch.cuda.synchronize()
-            return None, None
+            return None, None, []
 
     def capture_joint_step(self, mr_example, ct_example, keep_prob=0.75, warmup=2):
         """`d_step(mr, ct)` + `g_step(ct_g)` as ONE graph on static input buffers (the warm-up steps are real steps)."""
         self._gx_mr, self._gx_ct, self._gx_ct_g = mr_example.clone(), ct_example.clone(), ct_example.clone()
-        self._graph, self._graph_out = self._capture(
+        self._graph, self._graph_out, self._graph_bn = self._capture(
             lambda: (self.d_step(self._gx_mr, self._gx_ct, keep_prob), self.g_step(self._gx_ct_g, keep_prob)), warmup)
         self._graph_kp = keep_prob
         return self._graph is not None
@@ -607,13 +610,13 @@ class Trainer(object):
     def capture_d_step(self, mr_example, ct_example, keep_prob=0.75, warmup=2):
         """the discriminator update alone (pre-train phase; the n_D inner iterations of train-gan)"""
         self._dx_mr, self._dx_ct = mr_example.clone(), ct_example.clone()
-        self._d_graph, self._d_graph_out = self._capture(lambda: self.d_step(self._dx_mr, self._dx_ct, keep_prob), warmup)
+        self._d_graph, self._d_graph_out, self._d_graph_bn = self._capture(lambda: self.d_step(self._dx_mr, self._dx_ct, keep_prob), warmup)
         self._d_graph_kp = keep_prob
         return self._d_graph is not None
 
     def capture_g_step(self, ct_example, keep_prob=0.75, warmup=2):
         self._gsx_ct = ct_example.clone()
-        self._g_graph, self._g_graph_out = self._capture(lambda: self.g_step(self._gsx_ct, keep_prob), warmup)
+        self._g_graph, self._g_graph_out, self._g_graph_bn = self._capture(lambda: self.g_step(self._gsx_ct, keep_prob), warmup)
         self._g_graph_kp = keep_prob
         return self._g_graph is not None
 
@@ -624,7 +627,7 @@ class Trainer(object):
         self._dx_ct.copy_(ct_batch, non_blocking=True)
         self._d_graph.replay()
         self.global_step += 1
-        self.d_arena.bump_versions()
+        self._replayed(self._d_graph_bn, self.d_arena)
         return self._d_graph_out
 
     def g_step_replay(self, ct_batch, keep_prob=0.75):
@@ -633,11 +636,19 @@ class Trainer(object):
         self._gsx_ct.copy_(ct_batch, non_blocking=True)
         self._g_graph.replay()
         self.global_step += 1
-        self.g_arena.bump_versions()
+        self._replayed(self._g_graph_bn, self.g_arena)
         return self._g_graph_out
 
+    def _replayed(self, bn_moved, *arenas):
+        """a replay changed these arenas and moving statistics on the device: eager code that follows must not trust its cached
+        operands (weight planes, folded batch-norm coefficients)"""
+        for a in arenas:
+            a.bump_versions()
+        for v in bn_moved:
+            v.pnp_version += 1
+
     def release_graphs(self):
-        for n in ("_graph", "_graph_out", "_d_graph", "_d_graph_out", "_g_graph", "_g_graph_out"):
+        for n in ("_graph", "_graph_out", "_graph_bn", "_d_graph", "_d_graph_out", "_d_graph_bn", "_g_graph", "_g_graph_out", "_g_graph_bn"):
             setattr(self, n, None)
 
     def _invalidate_operand_caches(self):
@@ -656,9 +667,7 @@ class Trainer(object):
             self._gx_ct_g.copy_(ct_batch if ct_batch_g is None else ct_batch_g, non_blocking=True)
             self._graph.replay()
             self.global_step += 2
-            # the replay changed both arenas on the device: eager code that follows must not trust its cached operands
-            self.d_arena.bump_versions()
-            self.g_arena.bump_versions()
+            self._replayed(self._graph_bn, self.d_arena, self.g_arena)
             return self._graph_out
         return self.d_step(mr_batch, ct_batch, keep_prob), self.g_step(ct_batch if ct_batch_g is None else ct_batch_g, keep_prob)
 

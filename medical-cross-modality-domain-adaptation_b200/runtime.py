@@ -217,6 +217,18 @@ def global_variables():
     return [graph.vars[n] for n in graph.order]
 
 
+def moving_stat_versions():
+    """[(moving statistic, its version)]: taken before a CUDA-graph capture, see moving_stats_bumped_since"""
+    return [(v, v.pnp_version) for v in global_variables() if getattr(v, "pnp_kind", "") == "bn_moving"]
+
+
+def moving_stats_bumped_since(snapshot):
+    """the moving statistics whose version moved since `snapshot`, i.e. those of the batch norms that ran in training mode in
+    between.  A captured step bumps them on the host only while it is captured; a replay runs no host code, so whoever replays
+    bumps these (the coefficient cache of a batch norm with frozen gamma / beta keys on nothing else that changes)"""
+    return [v for v, ver in snapshot if v.pnp_version != ver]
+
+
 def state_dict():
     return {n: graph.vars[n].detach().cpu().numpy().copy() for n in graph.order}
 

@@ -97,7 +97,10 @@ class Full_DRN(object):
     def losses(self, logits, y):
         """(cost, weighted_loss, dice_loss) -- source_segmenter.py:211-273"""
         wce, dice = F.seg_losses(logits, y)
-        self.weighted_loss, self.dice_loss = wce, dice
+        # values only: a reference to the tensors themselves would keep the step's autograd graph alive, and with it the
+        # variables' gradient accumulators, which remember the stream they were created on.  A CUDA-graph capture that follows
+        # a step on another stream would then end its backward pass by waiting on that stream, which invalidates the capture
+        self.weighted_loss, self.dice_loss = wce.detach(), dice.detach()
         return wce, dice
 
     def cost_value(self, wce, dice):
@@ -193,7 +196,7 @@ class Trainer(object):
     def capture_train_step(self, x_example, y_example, keep_prob=0.75, warmup=2):
         """the Adam step as ONE CUDA graph on static input buffers (the warm-up steps are real steps)"""
         self._gx, self._gy = x_example.clone(), y_example.clone()
-        self._graph = None
+        self._graph = self._graph_out = None
         try:
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
@@ -206,10 +209,14 @@ class Trainer(object):
                 v.__dict__.pop("_pnp_planes", None)
                 v.__dict__.pop("_pnp_wT", None)
                 v.__dict__.pop("_pnp_bncoef", None)
+            before = rt.moving_stat_versions()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 out = self.train_step(self._gx, self._gy, keep_prob)
-            self._graph, self._graph_out, self._graph_kp = g, out, keep_prob
+            # (the losses are handed out detached, for the reason given in Full_DRN.losses: a later capture must not inherit
+            #  this one's gradient accumulators)
+            self._graph, self._graph_out, self._graph_kp = g, tuple(t.detach() for t in out), keep_prob
+            self._graph_bn = rt.moving_stats_bumped_since(before)
             return True
         except Exception as e:      # noqa: BLE001
             import warnings
@@ -226,6 +233,8 @@ class Trainer(object):
         self._graph.replay()
         self.global_step += 1
         self.arena.bump_versions()
+        for v in self._graph_bn:           # (with a frozen gamma / beta the arena's bump does not reach a batch norm's cache key)
+            v.pnp_version += 1
         return self._graph_out
 
     # scalar tags of the merged summary op, in its order (source_segmenter.py:387-396)

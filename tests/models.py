@@ -43,8 +43,9 @@ def adv_pair(backend, lam, phase, B, with_oracle=True, lr=3e-4, dis_sub_iter=1, 
     return net, trainer, oracle
 
 
-def seg_pair(backend, B, lr=1e-3, dtype=torch.float32):
-    """-> (net, trainer, oracle, initial variables); dtype: the oracle's"""
+def seg_pair(backend, B, lr=1e-3, dtype=torch.float32, optimizer="adam", **net_kw):
+    """-> (net, trainer, oracle, initial variables); dtype: the oracle's (which always steps with Adam and trains every variable);
+    net_kw: further arguments of the product's Full_DRN (main_trainable, adapt_trainable)"""
     import pnp_b200  # noqa: F401
     from pnp_b200 import runtime as rt, source_segmenter as seg
     from oracle.pnp_graphs import OracleSegmenter, init_numpy_params
@@ -53,9 +54,9 @@ def seg_pair(backend, B, lr=1e-3, dtype=torch.float32):
     P = init_numpy_params(ws, bns, 0, 0.05)
     bn_noise(P, bns, 5)
     ck = {"cross_flag": True, "miu_cross": 1.0, "dice_flag": True, "miu_dice": 1.0, "regularizer": 1e-4}
-    net = seg.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=dict(ck))
+    net = seg.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=dict(ck), **net_kw)
     rt.load_state_dict(P)
-    trainer = seg.Trainer(net, [], [], num_cls=5, batch_size=B, optimizer="adam", opt_kwargs={"learning_rate": lr})
+    trainer = seg.Trainer(net, [], [], num_cls=5, batch_size=B, optimizer=optimizer, opt_kwargs={"learning_rate": lr})
     return net, trainer, OracleSegmenter(P, B, dtype=dtype, lr=lr), P
 
 

@@ -455,6 +455,54 @@ def test_bucketed_overlapped_allreduce_gloo_world_size_2():
         assert out["err%d" % r] is not None and "more gradient contributions" in out["err%d" % r]
 
 
+def _version_worker(rank, world, port, out):
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
+    import torch.distributed as dist
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    import pnp_b200  # noqa: F401
+    from pnp_b200 import parallel, optim, layers as L, runtime as rt
+    rt.reset_default_graph()
+    torch.manual_seed(rank)                       # replicas start from different values
+    ws = [L.weight_variable([3, 3, 4, 8]), L.weight_variable([3, 3, 8, 8], trainable=False)]
+    bn = L.bn_variables("b", 8)
+    with torch.no_grad():
+        bn.moving_mean.fill_(float(rank))
+        bn.moving_var.fill_(1.0 + rank)
+    optim.Arena([ws[0], bn.gamma, bn.beta])       # arena members and free variables take different bump sites
+    names = list(rt.graph.order)
+    dp = parallel.DataParallel()
+    v0 = [rt.graph.vars[n].pnp_version for n in names]
+    dp.broadcast_variables(rt.global_variables())
+    v1 = [rt.graph.vars[n].pnp_version for n in names]
+    w_after = float(ws[1].flatten()[0])
+    with torch.no_grad():
+        bn.moving_mean.fill_(float(rank))
+    dp.average_moving_stats(rt.global_variables())
+    v2 = [rt.graph.vars[n].pnp_version for n in names]
+    out[rank] = (names, v0, v1, v2, w_after, float(bn.moving_mean[0]))
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+def test_data_parallel_writers_bump_every_version_gloo_world_size_2():
+    """the broadcast writes every variable (arena members through their arena, the others one by one) and the checkpoint's
+    statistics averaging writes every moving statistic: each written variable's pnp_version must be strictly larger afterwards,
+    or cached operands derived from the old values (weight planes, folded batch-norm coefficients) would be taken for current"""
+    import torch.multiprocessing as mp
+    mgr = mp.Manager()
+    out = mgr.dict()
+    mp.spawn(_version_worker, args=(2, 29900 + os.getpid() % 2000, out), nprocs=2, join=True)
+    for r in (0, 1):
+        names, v0, v1, v2, w_after, mm = out[r]
+        assert len(names) == 6 and out[r][4] == out[0][4] and mm == 0.5          # rank 0's weights, the mean of the statistics
+        for n, a, b, c in zip(names, v0, v1, v2):
+            assert b > a, "broadcast_variables left %s at version %d" % (n, a)
+            if "moving" in n:
+                assert c > b, "average_moving_stats left %s at version %d" % (n, b)
+            else:
+                assert c == b, n
+
+
 def test_entry_scripts_read_the_reference_list_files(tmp_path):
     """train_segmenter.py:60-61 / train_gan.py:69-72: `_read_lists` on ./lists/*_list (None when the file is absent, as in lib.py:11-12);
     a present list selects the TFRecord source of that stream -- training AND validation --, an absent one the synthetic source, and a
