@@ -60,8 +60,9 @@ def conv2d_raw(x, w, stride=1, dilation=1, padding="SAME"):
 
 
 def dropout(x, keep_prob, mask=None):
-    """tf.nn.dropout (layers.py:25,74,93): x * floor(keep + U) / keep.  TF's Philox stream is not
-    reproducible, so parity runs use keep_prob == 1 (identity) or an injected 0/1 mask."""
+    """tf.nn.dropout (layers.py:25,74,93): x * floor(keep + U) / keep, U from torch's generator here.  Parity runs use
+    keep_prob == 1 (identity), an injected 0/1 mask, or replace this function by tests/models.PhiloxMasks, which applies the
+    library's own Philox masks (tests/test_dropout_model_gpu.py)."""
     if mask is not None:
         return x * mask / keep_prob
     if keep_prob >= 1.0:

@@ -3,7 +3,7 @@ oracle on identical seeded initial variables, and the loss and variable comparis
 import numpy as np
 import torch
 
-from tests.util import rel_err
+from tests.util import l2_err, rel_err
 
 
 def bn_noise(P, bns, seed):
@@ -15,8 +15,9 @@ def bn_noise(P, bns, seed):
         P[n + "/moving_variance"] = (1 + 0.2 * rng.rand(c)).astype(np.float32)
 
 
-def adv_pair(backend, lam, phase, B, with_oracle=True, lr=3e-4, dis_sub_iter=1, o64=False):
-    """-> (net, trainer, oracle); o64: the oracle carries an fp64 companion as oracle.o64"""
+def adv_pair(backend, lam, phase, B, with_oracle=True, lr=3e-4, dis_sub_iter=1, o64=False, critic_keep_prob=1.0):
+    """-> (net, trainer, oracle); o64: the oracle carries an fp64 companion as oracle.o64; critic_keep_prob: both sides' critic
+    dropout (the reference hard-wires 0.75)"""
     import pnp_b200  # noqa: F401
     from pnp_b200 import runtime as rt, adversarial as adv
     from pnp_b200.train_gan import configure
@@ -31,12 +32,12 @@ def adv_pair(backend, lam, phase, B, with_oracle=True, lr=3e-4, dis_sub_iter=1, 
     ck, nc, tc = configure(phase)
     ck["lambda_mask_loss"] = lam
     tc["dis_sub_iter"] = dis_sub_iter
-    net = adv.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=ck, network_config=nc, critic_keep_prob=1.0)
+    net = adv.Full_DRN(channels=3, n_class=5, batch_size=B, cost_kwargs=ck, network_config=nc, critic_keep_prob=critic_keep_prob)
     rt.load_state_dict(P)
     trainer = adv.Trainer(net, num_cls=5, batch_size=B, opt_kwargs={"learning_rate": lr}, train_config=tc)
     oracle = None
     if with_oracle:
-        kw = dict(lambda_mask_loss=lam, dis_sub_iter=dis_sub_iter, gen_sub_iter=1, critic_keep_prob=1.0, lr=lr)
+        kw = dict(lambda_mask_loss=lam, dis_sub_iter=dis_sub_iter, gen_sub_iter=1, critic_keep_prob=critic_keep_prob, lr=lr)
         oracle = OracleAdversarial(P, B, **kw)
         if o64:
             oracle.o64 = OracleAdversarial(P, B, dtype=torch.float64, **kw)
@@ -58,6 +59,104 @@ def seg_pair(backend, B, lr=1e-3, dtype=torch.float32, optimizer="adam", **net_k
     rt.load_state_dict(P)
     trainer = seg.Trainer(net, [], [], num_cls=5, batch_size=B, optimizer=optimizer, opt_kwargs={"learning_rate": lr})
     return net, trainer, OracleSegmenter(P, B, dtype=dtype, lr=lr), P
+
+
+class PhiloxMasks:
+    """Stand-in for oracle.tf14_torch.dropout that applies the library's own dropout masks (oracle/philox.py), so that the oracle
+    can follow a training step with dropout on.  The masks come from the stream-id contract of runtime._Rng, not from the
+    product's state:
+      * manual_seed(S) stores s0 = S & (2^63 - 1); every executed step advances the seed once before its forward pass, so step
+        k (1-based, counting every D, G and segmenter step that runs kernels) reads seed_advance(s0, k);
+      * every dropout site with keep < 1 draws the next stream id, counting from 1 after manual_seed, in execution order.
+    Site n of the current step multiplies x by dropout_mult(seed, id, keep, x.numel()) laid over x's NHWC flat index, cast to x's
+    dtype (so an fp64 oracle multiplies by the exact fp32 values 0 and fl32(1/keep)).  keep >= 1 is the identity and draws no id.
+    Masks are cached by (seed, id, keep, n), so the fp32 and the fp64 oracle of one step see the same ones; moving to another
+    step drops the other seeds' masks (a B = 2 adversarial step draws ~70 M of them).  `seen` records the (shape, keep) of every
+    call."""
+
+    def __init__(self, seed):
+        self.s0 = int(seed) & 0x7FFFFFFFFFFFFFFF
+        self.k = 0          # the step whose seed the next site reads
+        self.sid = 0        # the last stream id drawn
+        self.cache = {}
+        self.seen = []
+
+    def at(self, k, sid):
+        """the next sites belong to step k and draw ids sid + 1, sid + 2, ..."""
+        self.k, self.sid = k, sid
+        s = self.seed()
+        self.cache = {key: v for key, v in self.cache.items() if key[0] == s}
+        return self
+
+    def seed(self, k=None):
+        from oracle import philox
+        return philox.seed_advance(self.s0, self.k if k is None else k)
+
+    def mult(self, seed, sid, keep, n):
+        """[n] fp32: dropout_mult(seed, sid, keep, n), the kept elements cached as a bool map"""
+        from oracle import philox
+        key = (seed, sid, float(keep), n)
+        if key not in self.cache:
+            self.cache[key] = torch.from_numpy(philox.dropout_mult(seed, sid, keep, n) != 0)
+        return torch.where(self.cache[key], torch.tensor(float(philox.inv_keep(keep))), torch.tensor(0.0))
+
+    def __call__(self, x, keep_prob, mask=None):
+        assert mask is None, "the stand-in draws its own mask"
+        self.seen.append((tuple(x.shape), float(keep_prob)))
+        if keep_prob >= 1.0:
+            return x
+        self.sid += 1
+        m = self.mult(self.seed(), self.sid, keep_prob, x.numel())
+        return x * m.reshape(x.shape).to(device=x.device, dtype=x.dtype)
+
+
+def grad_report(names, ours, g32, g64, slack=4.0, floor=2e-3):
+    """first-step gradients, variable by variable, in relative L2 against the fp64 oracle: the product may sit `slack` times as
+    far from fp64 as the fp32 oracle does (+ floor).  Returns (ours, fp32 oracle) worst errors"""
+    wp = wo = 0.0
+    for n, a, b32, b64 in zip(names, ours, g32, g64):
+        if float(b64.abs().max()) == 0.0:
+            assert float(a.abs().max()) == 0.0, n
+            continue
+        ep, eo = l2_err(a, b64), l2_err(b32, b64)
+        if ep > max(floor, slack * eo):
+            print("  grad %-40s l2 err %.3e (fp32 oracle %.3e)" % (n, ep, eo))
+        wp, wo = max(wp, ep), max(wo, eo)
+    print("  worst gradient l2 err vs fp64 oracle: ours %.3e, fp32 oracle %.3e" % (wp, wo))
+    assert wp <= slack * wo + floor, (wp, wo)
+    return wp, wo
+
+
+def snapshot(rt):
+    """every variable before a step (the weight-decay fold of adv_grads reads them)"""
+    return {n: rt.graph.vars[n].detach().cpu().clone() for n in rt.graph.order}
+
+
+def adv_grads(rt, oracle, which, pre):
+    """-> (names, the product's gradients of an adversarial step).  The optimizer's L2 term is folded into its kernel on our
+    side: wd * theta (theta from `pre`, the variables before the step) is added before comparing"""
+    if which == "d":
+        names = oracle.cls_w + [n + "/" + l for n in oracle.cls_bn for l in ("gamma", "beta")]
+        wd = {n: oracle.gan_reg * oracle.miu_dis * 2.0 / oracle.dis_sub_iter * (1.0 if n.startswith("cls_scope") else oracle.lam)
+              for n in oracle.cls_w}
+    else:
+        names = oracle.adapt_w + [n + "/" + l for n in oracle.adapt_bn for l in ("gamma", "beta")]
+        wd = {n: oracle.gan_reg * oracle.miu_gen / oracle.gen_sub_iter for n in oracle.adapt_w}
+    ours = []
+    for n in names:
+        a = rt.graph.vars[n].grad.cpu().double()
+        if n in wd:
+            a = a + wd[n] * pre[n].double()
+        ours.append(a)
+    return names, ours
+
+
+def compare_adv_grads(rt, oracle, which, g32, g64, pre, backend="simt"):
+    """first-step gradients of an adversarial step against the fp64 oracle.  fp32 SIMT path: as accurate as an fp32 reference
+    (slack 4); the bf16-split tensor-core path carries ~1e-5 per conv instead of ~1e-7, amplified by the same BN-backward
+    cancellation: slack 10"""
+    names, ours = adv_grads(rt, oracle, which, pre)
+    return grad_report(names, ours, g32, g64, slack=4.0 if backend == "simt" else 10.0)
 
 
 def loss_close(name, got, ref, scale_floor, tol=1e-3):

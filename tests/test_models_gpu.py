@@ -5,12 +5,13 @@ synthetic 256x256x3 inputs and identical initial variables (loaded by TF variabl
   config 3: D step (pre-train, lambda=0) + clip -> dis_loss, critic logits, updated variables
   config 4: D step + G step (train-gan, lambda=0.3)
 Tolerance (BASELINE.json north_star): 1e-3 relative fp32, stated per check; dropout off (keep_prob=1,
-critic_keep_prob=1) because TF's Philox stream cannot be reproduced (SURVEY App. B.4).
+critic_keep_prob=1).  The same steps with dropout on, the oracle applying the library's own Philox masks, are
+tests/test_dropout_model_gpu.py.
 """
 import pytest
 import torch
 
-from tests.models import adv_pair, seg_pair, state_close
+from tests.models import adv_pair, compare_adv_grads, grad_report, seg_pair, snapshot, state_close
 from tests.util import check, rel_err, l2_err
 
 pytestmark = pytest.mark.gpu
@@ -68,7 +69,7 @@ def test_config2_segmenter_train_step(backend):
         check("step%d dice" % step, dice.reshape(1), torch.tensor([ro["dice"]]), 1e-3)
         if step == 0:
             # first-step gradients, variable by variable, against the fp64 oracle; bound calibrated by how far an fp32
-            # reference implementation (the fp32 oracle) itself sits from fp64 on this ill-conditioned backward pass
+            # reference implementation (the fp32 oracle) itself sits from fp64 on this ill-conditioned backward pass (grad_report)
             names = [n for n, _ in type(oracle).layout()[0]]
             bn_names = [n for n, _ in type(oracle).layout()[1]]
             all_names = names + [n + "/" + l for n in bn_names for l in ("gamma", "beta")]
@@ -77,7 +78,7 @@ def test_config2_segmenter_train_step(backend):
                 v = rt.graph.vars[n]
                 mult = sum(1 for w in net.conv_weights if w is v)
                 ours.append(v.grad.cpu().double() + 1e-4 * mult * torch.tensor(P[n]).double())
-            _grad_report(all_names, ours, ro["grads"], g64, slack=4.0 if backend == "simt" else 10.0)
+            grad_report(all_names, ours, ro["grads"], g64, slack=4.0 if backend == "simt" else 10.0)
     # Adam's first updates are ~ lr*sign(g): elements whose gradient sits below the fp32 noise floor of this backward pass
     # (see _grad_report) may step the other way, so variables are compared in relative L2 (a few 1e-3 of the elements
     # moving by 2*lr), not max-norm; the per-step losses above are the end-to-end check at 1e-3
@@ -87,50 +88,6 @@ def test_config2_segmenter_train_step(backend):
     rt.set_conv_backend("auto")
 
 
-def _grad_report(names, ours, g32, g64, slack=4.0, floor=2e-3):
-    wp = wo = 0.0
-    for n, a, b32, b64 in zip(names, ours, g32, g64):
-        if float(b64.abs().max()) == 0.0:
-            assert float(a.abs().max()) == 0.0, n
-            continue
-        ep, eo = l2_err(a, b64), l2_err(b32, b64)
-        if ep > max(floor, slack * eo):
-            print("  grad %-40s l2 err %.3e (fp32 oracle %.3e)" % (n, ep, eo))
-        wp, wo = max(wp, ep), max(wo, eo)
-    print("  worst gradient l2 err vs fp64 oracle: ours %.3e, fp32 oracle %.3e" % (wp, wo))
-    assert wp <= slack * wo + floor, (wp, wo)
-
-
-def _compare_grads(rt, oracle, which, g32, g64, backend="simt"):
-    """first-step gradients of an adversarial step, variable by variable (the optimizer's L2 term is folded into its
-    kernel on our side: add wd*theta before comparing)"""
-    if which == "d":
-        names = oracle.cls_w + [n + "/" + l for n in oracle.cls_bn for l in ("gamma", "beta")]
-        wd = {n: oracle.gan_reg * oracle.miu_dis * 2.0 / oracle.dis_sub_iter * (1.0 if n.startswith("cls_scope") else oracle.lam)
-              for n in oracle.cls_w}
-    else:
-        names = oracle.adapt_w + [n + "/" + l for n in oracle.adapt_bn for l in ("gamma", "beta")]
-        wd = {n: oracle.gan_reg * oracle.miu_gen / oracle.gen_sub_iter for n in oracle.adapt_w}
-    ours = []
-    for n in names:
-        a = rt.graph.vars[n].grad.cpu().double()
-        if n in wd:
-            a = a + wd[n] * PRE[n].double()
-        ours.append(a)
-    # fp32 SIMT path: as accurate as an fp32 reference (slack 4); the bf16-split tensor-core path carries ~1e-5 per conv
-    # instead of ~1e-7, amplified by the same BN-backward cancellation: slack 10
-    _grad_report(names, ours, g32, g64, slack=4.0 if backend == "simt" else 10.0)
-
-
-PRE = {}
-
-
-def _snapshot(rt):
-    PRE.clear()
-    for n in rt.graph.order:
-        PRE[n] = rt.graph.vars[n].detach().cpu().clone()
-
-
 @pytest.mark.parametrize("backend", ["simt", "auto"])
 def test_config3_discriminator_pretrain_step(backend):
     from pnp_b200 import runtime as rt
@@ -138,11 +95,12 @@ def test_config3_discriminator_pretrain_step(backend):
     net, trainer, oracle = adv_pair(backend, 0, "pre-train", B, dis_sub_iter=3, o64=True)
     mr, ct = synthetic_images(B, 1234), synthetic_images(B, 4321, 0.3, 0.8)
     for step in range(2):
-        _snapshot(rt)
+        pre = snapshot(rt)
         ro = oracle.d_step(mr, ct, keep_prob=1.0)
         terms = trainer.d_step(mr.to(DEV), ct.to(DEV), keep_prob=1.0)
         if step == 0:
-            _compare_grads(rt, oracle, "d", ro["grads"], oracle.o64.d_step(mr.double(), ct.double(), keep_prob=1.0)["grads"], backend)
+            compare_adv_grads(rt, oracle, "d", ro["grads"], oracle.o64.d_step(mr.double(), ct.double(), keep_prob=1.0)["grads"], pre,
+                              backend)
         got = trainer.loss_value(terms)
         print("  step %d dis_loss %.6e (oracle %.6e)" % (step, got, ro["dis_loss"]))
         assert abs(got - ro["dis_loss"]) <= 1e-3 * max(abs(ro["dis_loss"]), 2e-3 * float(ro["mr_cls"].abs().max()))
@@ -157,17 +115,17 @@ def test_config4_joint_adversarial_step(backend):
     from oracle.pnp_graphs import synthetic_images
     net, trainer, oracle = adv_pair(backend, 0.3, "train-gan", B, dis_sub_iter=3, o64=True)
     mr, ct = synthetic_images(B, 1234), synthetic_images(B, 4321, 0.3, 0.8)
-    _snapshot(rt)
+    pre = snapshot(rt)
     ro = oracle.d_step(mr, ct, keep_prob=1.0)
     terms = trainer.d_step(mr.to(DEV), ct.to(DEV), keep_prob=1.0)
-    _compare_grads(rt, oracle, "d", ro["grads"], oracle.o64.d_step(mr.double(), ct.double(), keep_prob=1.0)["grads"], backend)
+    compare_adv_grads(rt, oracle, "d", ro["grads"], oracle.o64.d_step(mr.double(), ct.double(), keep_prob=1.0)["grads"], pre, backend)
     got = trainer.loss_value(terms)
     print("  dis_loss %.6e (oracle %.6e)" % (got, ro["dis_loss"]))
     assert abs(got - ro["dis_loss"]) <= 1e-3 * max(abs(ro["dis_loss"]), 2e-3 * float(ro["mr_cls"].abs().max()))
-    _snapshot(rt)
+    pre = snapshot(rt)
     rg = oracle.g_step(ct, keep_prob=1.0)
     terms = trainer.g_step(ct.to(DEV), keep_prob=1.0)
-    _compare_grads(rt, oracle, "g", rg["grads"], oracle.o64.g_step(ct.double(), keep_prob=1.0)["grads"], backend)
+    compare_adv_grads(rt, oracle, "g", rg["grads"], oracle.o64.g_step(ct.double(), keep_prob=1.0)["grads"], pre, backend)
     got = trainer.loss_value(terms)
     print("  gen_loss %.6e (oracle %.6e)" % (got, rg["gen_loss"]))
     assert abs(got - rg["gen_loss"]) <= 1e-3 * max(abs(rg["gen_loss"]), 2e-3 * float(rg["ct_cls"].abs().max()))

@@ -8,7 +8,9 @@ seeded synthetic inputs and identical initial variables:
   config 5: the plain-bf16 (one MMA term) path -- its model-level deviation from the fp32 reference, stated and bounded
   CUDA graph vs eager with the critic weights perturbed between steps (a graph running on stale operands cannot pass)
 
-Tolerance (BASELINE.json north_star): 1e-3 relative, written at each check.  Dropout off (TF's Philox stream cannot be reproduced).
+Tolerance (BASELINE.json north_star): 1e-3 relative, written at each check.  Dropout off; the benchmarked keep 0.75, eager and
+graph-replayed (B = 8 joint replay included), is held to the oracle fed the library's own Philox masks in
+tests/test_dropout_model_gpu.py.
 """
 import pytest
 import torch

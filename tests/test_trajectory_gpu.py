@@ -22,6 +22,9 @@
     class, per batch and in the mean.  The checkpoint evaluated is the first one on which hard Dice is insensitive to fp32
     rounding (measured oracle-free, between the product's wgmma and SIMT convolution paths): a model with thousands of
     pixels within rounding of a tie separates no two fp32 implementations to 1e-3 (see the comment in the test).
+
+Dropout is off in every run here (keep 1, critic keep 1); the steps with dropout on, against an oracle that applies the library's
+own Philox masks, are tests/test_dropout_model_gpu.py.
 """
 import json
 import os
