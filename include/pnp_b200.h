@@ -320,6 +320,29 @@ int pnp_surface_distance_workspace(int n0, int n1, int n2, int C, long long* byt
 int pnp_surface_distance(const uint8_t* pred, const uint8_t* gt, int n0, int n1, int n2, int C, const double* spacing /* host, 3 */,
                          void* ws, long long ws_bytes, double* out, void* stream);
 
+/* ---- data preparation: planes resampled out of a volume (resample.cu) ----------------------------------------------------------
+ * The augmented coronal slices of the data preparation (preprocess.py; the reference only describes it, README step 1) in one launch
+ * per batch.  vol is fp32 and cls uint8 class ids, both C-order [n0][n1][n2] (n2 fastest) on the device.  Output plane p = b*C + k
+ * has its own 3 x 3 matrix m = mats[9p .. 9p+8] (row-major, device); pixel (r, c) of plane p samples the source coordinate
+ *   u_i = (m_i0 * r + m_i1 * c) + m_i2,   i = 0, 1, 2,
+ * each product and each sum rounded separately in fp32 (no FMA contraction).
+ *   img[b][r][c][k] (fp32 [B,H,W,C]): trilinear interpolation of vol.  Each u_i is clamped into [0, n_i - 1]; i0 = floor(u),
+ *     i1 = min(i0 + 1, n_i - 1), f = u - i0; interpolation runs along axis 2, then 1, then 0, each step a + f*(b - a) with every
+ *     operation rounded.  A NaN coordinate clamps to 0.
+ *   lab (int64): the nearest voxel floor(u_i + 0.5) of cls (ties round up); class 0 when any u_i < -0.5, u_i >= n_i - 0.5 or
+ *     u_i is NaN.  label_planes = 1 writes plane C/2 only, as lab[b][r][c] ([B,H,W], what the trainers consume); label_planes = C
+ *     writes every plane, lab[b][r][c][k] ([B,H,W,C], what the record writer stores); 0 writes no labels.
+ * A prepared test volume [H, W, D] is the call with B = 1 and C = D: NHWC with B = 1 is the NIfTI C-order layout.
+ *
+ * img may be NULL (labels only); vol may then be NULL too, and cls / lab may be NULL with label_planes = 0.  NULL mats, a NULL
+ * pointer an output needs, no output at all or a non-positive size are PNP_ERR_BAD_ARG; label_planes other than 0, 1 or C, a
+ * dimension n_i, H or W above PNP_RS_MAX_DIM (fp32 coordinates must resolve every voxel and n - 0.5 must be exact) or
+ * n0*n1*n2, B*H*W*C or B*C*9 >= 2^31 are PNP_ERR_UNSUPPORTED.  On any error nothing is launched and the outputs are untouched.
+ * Every output element is written once by one thread, so repeated calls are bit-identical. */
+#define PNP_RS_MAX_DIM (1 << 23)
+int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W, int C,
+                        float* img, long long* lab, int label_planes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

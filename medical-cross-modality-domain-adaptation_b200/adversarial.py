@@ -318,7 +318,8 @@ class Trainer(object):
 
     def __init__(self, net, mr_train_list=None, mr_val_list=None, ct_train_list=None, ct_val_list=None, adapt_var_list=None,
                  mr_var_list=None, old_bn_list=None, new_bn_list=None, test_label_list=None, test_nii_list=None, num_cls=None,
-                 batch_size=6, opt_kwargs={}, train_config={}, mr_source=None, ct_source=None):
+                 batch_size=6, opt_kwargs={}, train_config={}, mr_source=None, ct_source=None, mr_val_source=None,
+                 ct_val_source=None):
         self.net = net
         self.batch_size = batch_size
         self.num_cls = num_cls
@@ -326,6 +327,7 @@ class Trainer(object):
         self.train_config = dict(train_config)
         self.lr_update_flag = self.train_config.get("lr_update", False)
         self.mr_source, self.ct_source = mr_source, ct_source
+        self.mr_val_source, self.ct_val_source = mr_val_source, ct_val_source
         self.mr_train_list, self.ct_train_list = mr_train_list, ct_train_list
         self.mr_val_list, self.ct_val_list = mr_val_list, ct_val_list
         self.test_label_list, self.test_nii_list = test_label_list, test_nii_list
@@ -743,9 +745,9 @@ class Trainer(object):
             return SyntheticSource(B, seed=seed + self.dp.rank, num_cls=self.num_cls or 5, **kw)
         mr_src = source(self.mr_source, self.mr_train_list, 1234)
         ct_src = source(self.ct_source, self.ct_train_list, 4321, shift=0.3, scale=0.8)
-        # the validation queues of adversarial.py:811-815 (lists/{mr,ct}_val_list), else further synthetic streams
-        mr_val = source(None, self.mr_val_list, 2234)
-        ct_val = source(None, self.ct_val_list, 5321, shift=0.3, scale=0.8)
+        # the validation queues of adversarial.py:811-815: the given sources, else lists/{mr,ct}_val_list, else further synthetic streams
+        mr_val = source(self.mr_val_source, self.mr_val_list, 2234)
+        ct_val = source(self.ct_val_source, self.ct_val_list, 5321, shift=0.3, scale=0.8)
         dev = rt.device()
         dis_interval, gen_interval = cfg.get("dis_interval", 1), cfg.get("gen_interval", 1)
         dis_inc, gen_inc = cfg.get("dis_sub_iter_inc", 0), cfg.get("gen_sub_iter_inc", 0)

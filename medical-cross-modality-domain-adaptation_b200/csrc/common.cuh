@@ -25,6 +25,14 @@
 
 static inline int pnp_cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// grid of a grid-stride kernel: one CTA per per_block work items, at least 1, at most 64 per SM
+static inline int grid_for(long long work_items, int per_block) {
+  long long b = (work_items + per_block - 1) / per_block;
+  if (b < 1) b = 1;
+  if (b > PNP_NUM_SMS * 64LL) b = PNP_NUM_SMS * 64LL;
+  return (int)b;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Programmatic dependent launch (opt-in: PNP_PDL=1).  A step is ~860 short kernels in stream order (inside one CUDA graph).
 // Every kernel of this library starts with pnp_pdl_enter(): `griddepcontrol.launch_dependents` lets the NEXT kernel of the

@@ -48,13 +48,6 @@ __device__ __forceinline__ float act_slope(float y, int act) {
   return 1.f;
 }
 
-inline int grid_for(long long work_items, int per_block) {
-  long long b = (work_items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > PNP_NUM_SMS * 64LL) b = PNP_NUM_SMS * 64LL;
-  return (int)b;
-}
-
 PnpDropout make_drop(const pnp_dropout_cfg* d) { return pnp_make_drop(d); }
 
 // ------------------------------------------------------------------------------------------------
@@ -1604,4 +1597,4 @@ extern "C" const char* pnp_error_string(int code) {
   }
 }
 
-extern "C" int pnp_version(void) { return 102; }
+extern "C" int pnp_version(void) { return 103; }

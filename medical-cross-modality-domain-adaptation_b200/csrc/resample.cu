@@ -1,0 +1,104 @@
+// Planes resampled out of a device-resident volume: the data-preparation hot path (preprocess.py).  One launch draws every
+// augmented coronal slice of a batch -- images by trilinear interpolation of the z-scored intensities, labels by the nearest voxel
+// of the class-id volume -- straight into the trainers' NHWC layout, so a trainer can draw fresh augmentations every step
+// without record files or a host-to-device image copy.  A grid-stride gather: the writes are coalesced along the NHWC index,
+// the reads follow the sampled coordinates.
+#include "common.cuh"
+#include "../../include/pnp_b200.h"
+
+#include <initializer_list>
+
+namespace {
+
+// a + f (b - a) with each operation rounded (no FMA contraction): the host restatement (oracle/resample_exact.py) computes
+// the same three roundings
+__device__ __forceinline__ float lerp_rn(float a, float b, float f) { return __fadd_rn(a, __fmul_rn(f, __fsub_rn(b, a))); }
+
+// trilinear taps along one axis: clamp into [0, n - 1], i0 = floor, i1 = min(i0 + 1, n - 1), f = x - i0 (exact for x >= 0).
+// fmaxf sends a NaN coordinate to 0.
+__device__ __forceinline__ void axis_taps(float u, int n, int& i0, int& i1, float& f) {
+  const float x = fminf(fmaxf(u, 0.f), (float)(n - 1));
+  const float fl = floorf(x);
+  i0 = (int)fl;
+  i1 = min(i0 + 1, n - 1);
+  f = __fsub_rn(x, fl);
+}
+
+// nearest voxel floor(u + 0.5) (ties round up), -1 outside [-0.5, n - 0.5) or for a NaN coordinate.  n <= 2^23 keeps n - 0.5
+// exact; the min() only guards the index.
+__device__ __forceinline__ int axis_nearest(float u, int n) {
+  if (!(u >= -0.5f && u < __fsub_rn((float)n, 0.5f))) return -1;
+  return min((int)floorf(__fadd_rn(u, 0.5f)), n - 1);
+}
+
+// Item q of the NHWC output: k = q % Cw (or C / 2 when only the middle label plane is written, Cw == 1), pixel = q / Cw.
+__global__ void __launch_bounds__(256)
+resample_planes_kernel(const float* __restrict__ vol, const uint8_t* __restrict__ cls, int n0, int n1, int n2,
+                       const float* __restrict__ mats, int H, int W, int C, int Cw, long long total, float* __restrict__ img,
+                       long long* __restrict__ lab, int label_planes) {
+  pnp_pdl_enter();
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const unsigned q = (unsigned)i;
+    const int k = Cw == C ? (int)(q % (unsigned)C) : C / 2;
+    const unsigned pix = q / (unsigned)Cw;                  // (b H + r) W + c
+    const unsigned row = pix / (unsigned)W;
+    const int c = (int)(pix - row * (unsigned)W), r = (int)(row % (unsigned)H), b = (int)(row / (unsigned)H);
+    const float* m = mats + (long long)(b * C + k) * 9;
+    const float fr = (float)r, fc = (float)c;
+    float u[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) u[a] = __fadd_rn(__fadd_rn(__fmul_rn(__ldg(m + 3 * a), fr), __fmul_rn(__ldg(m + 3 * a + 1), fc)),
+                                                 __ldg(m + 3 * a + 2));
+    const long long o = (long long)pix * C + k;
+    if (img) {
+      int a0, b0, a1, b1, a2, b2;
+      float f0, f1, f2;
+      axis_taps(u[0], n0, a0, b0, f0);
+      axis_taps(u[1], n1, a1, b1, f1);
+      axis_taps(u[2], n2, a2, b2, f2);
+      const float* p00 = vol + (a0 * n1 + a1) * n2;
+      const float* p01 = vol + (a0 * n1 + b1) * n2;
+      const float* p10 = vol + (b0 * n1 + a1) * n2;
+      const float* p11 = vol + (b0 * n1 + b1) * n2;
+      const float v00 = lerp_rn(__ldg(p00 + a2), __ldg(p00 + b2), f2);
+      const float v01 = lerp_rn(__ldg(p01 + a2), __ldg(p01 + b2), f2);
+      const float v10 = lerp_rn(__ldg(p10 + a2), __ldg(p10 + b2), f2);
+      const float v11 = lerp_rn(__ldg(p11 + a2), __ldg(p11 + b2), f2);
+      img[o] = lerp_rn(lerp_rn(v00, v01, f1), lerp_rn(v10, v11, f1), f0);
+    }
+    if (label_planes) {
+      const int j0 = axis_nearest(u[0], n0), j1 = axis_nearest(u[1], n1), j2 = axis_nearest(u[2], n2);
+      const long long v = (j0 < 0 || j1 < 0 || j2 < 0) ? 0LL : (long long)__ldg(cls + (j0 * n1 + j1) * n2 + j2);
+      if (label_planes == C) lab[o] = v;
+      else if (k == C / 2) lab[pix] = v;
+    }
+  }
+}
+
+// a product of positive ints below 2^31 (each factor is, so no partial product overflows)
+bool count_below_2_31(std::initializer_list<int> dims) {
+  long long n = 1;
+  for (int d : dims) {
+    n *= d;
+    if (n >= (1LL << 31)) return false;
+  }
+  return true;
+}
+
+}  // namespace
+
+extern "C" int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W,
+                                   int C, float* img, long long* lab, int label_planes, void* stream) {
+  if (!mats || n0 <= 0 || n1 <= 0 || n2 <= 0 || B <= 0 || H <= 0 || W <= 0 || C <= 0) return PNP_ERR_BAD_ARG;
+  if (label_planes != 0 && label_planes != 1 && label_planes != C) return PNP_ERR_UNSUPPORTED;
+  if (!img && !label_planes) return PNP_ERR_BAD_ARG;
+  if ((img && !vol) || (label_planes && (!cls || !lab))) return PNP_ERR_BAD_ARG;
+  if (n0 > PNP_RS_MAX_DIM || n1 > PNP_RS_MAX_DIM || n2 > PNP_RS_MAX_DIM || H > PNP_RS_MAX_DIM || W > PNP_RS_MAX_DIM)
+    return PNP_ERR_UNSUPPORTED;
+  if (!count_below_2_31({n0, n1, n2}) || !count_below_2_31({B, H, W, C}) || !count_below_2_31({B, C, 9})) return PNP_ERR_UNSUPPORTED;
+  const int Cw = (img || label_planes != 1) ? C : 1;
+  const long long total = (long long)B * H * W * Cw;
+  PNP_CUDA(pnp_launch(resample_planes_kernel, grid_for(total, 256 * 4), 256, 0, (cudaStream_t)stream, vol, cls, n0, n1, n2, mats, H, W,
+                      C, Cw, total, img, lab, label_planes));
+  return PNP_OK;
+}

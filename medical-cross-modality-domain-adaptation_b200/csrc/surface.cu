@@ -7,13 +7,6 @@
 
 namespace {
 
-inline int grid_for(long long work_items, int per_block) {
-  long long b = (work_items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > PNP_NUM_SMS * 64LL) b = PNP_NUM_SMS * 64LL;
-  return (int)b;
-}
-
 // TF 'SAME' pooling geometry with ksize = stride = n: Ho = ceil(H / n), pad_total = Ho * n - H (< n), pad_before = pad_total / 2;
 // window `o` covers input rows [o * n - pad_before, o * n - pad_before + n) clipped to the image (padding never wins a max and is not
 // counted by the average).  Every input row belongs to exactly one window: o = (i + pad_before) / n.

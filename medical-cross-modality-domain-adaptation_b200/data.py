@@ -49,5 +49,58 @@ class SyntheticSource:
         return item
 
 
+class VolumeSource:
+    """Augmented training slices drawn straight from MMWHS volumes on the device (preprocess.py): next() returns (images
+    [B,256,256,3] fp32, labels [B,256,256] int64) like TFRecordSource.next(), but already on the device, so the trainers'
+    to_device is a no-op.  Every subject of `pairs` ((image_path, label_path) NIfTI pairs) is prepared once and its sub-volume
+    uploaded; each next() draws per sample a subject, a slice and (augment=True) an augmentation from
+    np.random.RandomState(seed), and resamples the whole batch in one pnp_resample_planes launch.  A batch stays valid until
+    the next-but-one call (two alternating output buffers, like TFRecordSource's)."""
+
+    def __init__(self, pairs, batch_size, seed, augment=True):
+        from . import preprocess
+        from . import runtime as rt
+        pairs = list(pairs)
+        if not pairs:
+            raise ValueError("empty volume list")
+        self.B, self.augment = batch_size, augment
+        self.subjects = [preprocess.Subject(im, lb) for im, lb in pairs]
+        vol, cls, self.offsets = preprocess.stack(self.subjects)
+        dev = rt.device()
+        self.vol, self.cls = torch.from_numpy(vol).to(dev), torch.from_numpy(cls).to(dev)
+        self.rng = np.random.RandomState(seed)
+        S = preprocess.SIZE
+        self._out = [(torch.empty(batch_size, S, S, 3, dtype=torch.float32, device=dev),
+                      torch.empty(batch_size, S, S, dtype=torch.int64, device=dev)) for _ in range(2)]
+        self._mats = [torch.empty(batch_size, 3, 3, 3, dtype=torch.float32, device=dev) for _ in range(2)]
+        # the matrices go up from pinned memory without stalling the stream; an event says when a host buffer is free again
+        self._host = [torch.empty(batch_size, 3, 3, 3, dtype=torch.float32, pin_memory=True) for _ in range(2)]
+        self._copied = [None, None]
+        self._flip = 0
+
+    def draw_matrices(self):
+        """fp32 [B, 3, 3, 3]: the matrices of the channels j - 1, j, j + 1 of B samples drawn from the generator"""
+        mats = []
+        for _ in range(self.B):
+            s = int(self.rng.randint(len(self.subjects)))
+            j, T = self.subjects[s].draw(self.rng, self.augment)
+            mats.append(self.subjects[s].matrices((j - 1, j, j + 1), T, self.offsets[s]))
+        return np.stack(mats)
+
+    def next(self):
+        from .functional import resample_planes
+        i = self._flip
+        self._flip ^= 1
+        x, y = self._out[i]
+        if self._copied[i] is not None:
+            self._copied[i].synchronize()
+        self._host[i].numpy()[...] = self.draw_matrices()
+        self._mats[i].copy_(self._host[i], non_blocking=True)
+        self._copied[i] = torch.cuda.Event()
+        self._copied[i].record()
+        resample_planes(self.vol, self.cls, self._mats[i], x.shape[1], x.shape[2], True, 1, x, y)
+        return x, y
+
+
 def to_device(x, dev):
     return x.to(dev, non_blocking=True)

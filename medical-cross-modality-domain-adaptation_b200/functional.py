@@ -1076,6 +1076,23 @@ def surface_from_raw(raw):
     return res
 
 
+def resample_planes(vol, cls, mats, H, W, image=True, label_planes=1, img=None, lab=None):
+    """Planes resampled out of a device volume in one pnp_resample_planes launch (include/pnp_b200.h, "data preparation").
+    `vol` fp32 and `cls` uint8 [n0, n1, n2] (either may be None when its output is not wanted), `mats` fp32 [B, C, 3, 3] on the
+    device.  Returns (img fp32 [B, H, W, C] or None, lab int64 [B, H, W] (label_planes 1), [B, H, W, C] (label_planes C) or None);
+    `img` / `lab` may be given to write into."""
+    B, C = mats.shape[0], mats.shape[1]
+    ref = vol if vol is not None else cls
+    n0, n1, n2 = ref.shape
+    if image and img is None:
+        img = torch.empty(B, H, W, C, dtype=torch.float32, device=ref.device)
+    if label_planes and lab is None:
+        lab = torch.empty((B, H, W) if label_planes == 1 else (B, H, W, C), dtype=torch.int64, device=ref.device)
+    call("pnp_resample_planes", ptr(vol), ptr(cls), n0, n1, n2, ptr(mats), B, H, W, C, ptr(img) if image else None,
+         ptr(lab) if label_planes else None, label_planes, rt.stream())
+    return (img if image else None), (lab if label_planes else None)
+
+
 def confusion_counts(logits, y):
     """[C,C] int64 confusion matrix (rows = truth) of argmax(logits) vs one-hot y (lib.py:96-110)."""
     logits, y = logits.contiguous(), y.contiguous()

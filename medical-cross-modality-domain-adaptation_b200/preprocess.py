@@ -1,0 +1,246 @@
+"""Data preparation of the MMWHS challenge volumes: step 1 of the reference's README (crop around the heart, cut the top 2 % of
+each volume's intensity histogram, z-score each volume, sample 2-D coronal slices with data augmentation and 3 neighbouring
+slices as channels).  The reference describes these steps but ships no code for them, so every choice below that its README does
+not fix is this project's own: the coronal frame, the crop margin, the augmentation ranges and the label table (DESIGN 6.1).
+
+Host side, in fp64 numpy:
+* labels: MMWHS values 205 / 420 / 500 / 820 -> classes 1 / 2 / 3 / 4 of evaluation.contour_map (LV myocardium, LA blood, LV
+  blood, ascending aorta); every other value -> 0.  Voxels holding a value outside the MMWHS set are counted and logged.
+* orientation: the nearest signed axis permutation to RAS+ of the NIfTI affine (nifti.header_affine), as nibabel's
+  io_orientation chooses it; spacing from the affine's column norms.  Coronal frame: rows run superior -> inferior, columns from the
+  patient's right to left (radiological), slices anterior -> posterior.  The largest angle between a voxel axis and its world axis
+  is logged: oblique volumes are resampled along the nearest permutation, not along their true axes.
+* crop: the bounding box of every non-zero MMWHS label (the whole heart) in mm.  The in-plane square of side (1 + 2 margin) times
+  the larger in-plane extent maps to 256 x 256 pixels; output voxels are isotropic at that pixel size, so the channels j - 1, j,
+  j + 1 are one pixel apart, and D slices cover the box's anterior-posterior extent plus the margin.
+* intensity: over the raw voxels inside the box, p98 = np.percentile(., 98) (linear), then mu and the population sigma of
+  min(x, p98); the device volume is (min(x, p98) - mu) / sigma, computed in fp64 and rounded to fp32 once.  Only the box plus the
+  largest displacement an augmentation can reach is uploaded, with the volume's edge voxels repeated beyond its border (what
+  clamping the coordinate into the whole volume would read) and class 0 there.
+* augmentation, per sample: slice j uniform over the heart's slice range, then a rotation U(-15, 15) degrees about the crop
+  centre, a scale U(0.9, 1.1) per in-plane axis and a translation U(-10, 10) pixels per axis, from a seeded np.random.RandomState;
+  output pixel p samples the un-augmented frame at centre + t + R(theta) S (p - centre).  Matrices are composed in fp64 and
+  rounded to fp32 once.  augment=False: the identity at every slice.
+
+The device side is one pnp_resample_planes launch per batch (functional.resample_planes)."""
+import logging
+import math
+import os
+
+import numpy as np
+
+from . import nifti
+
+MMWHS_VALUES = (205, 420, 500, 550, 600, 820, 850)
+LABEL_TABLE = {205: 1, 420: 2, 500: 3, 820: 4}       # MMWHS value -> evaluation.contour_map class
+SIZE = 256                                           # output planes are SIZE x SIZE
+MARGIN = 0.1
+ROTATION_DEG = 15.0
+SCALE_RANGE = (0.9, 1.1)
+SHIFT_PX = 10.0
+# RAS+ world axis and direction of the coronal frame's axes: rows S -> I (-z), columns R -> L (-x), slices A -> P (-y)
+FRAME = ((2, -1), (0, -1), (1, -1))
+CENTRE = (SIZE - 1) / 2.0
+# the farthest an augmented pixel samples from the crop centre, in output pixels
+REACH_PX = SCALE_RANGE[1] * math.hypot(CENTRE, CENTRE) + math.hypot(SHIFT_PX, SHIFT_PX)
+
+
+def map_labels(raw):
+    """MMWHS label values -> (uint8 class ids, boolean whole-heart mask, number of voxels outside {0} and the MMWHS set)"""
+    raw = np.asarray(raw)
+    out = np.zeros(raw.shape, np.uint8)
+    for v, c in LABEL_TABLE.items():
+        out[raw == v] = c
+    heart = np.isin(raw, MMWHS_VALUES)
+    unknown = int(raw.size - heart.sum() - (raw == 0).sum())
+    return out, heart, unknown
+
+
+def orientation(affine):
+    """voxel axis v -> (RAS+ world axis, sign) of the nearest signed axis permutation, the voxel spacing and the largest angle
+    (degrees) between a voxel axis and its world axis.  Like nibabel's io_orientation: the column-normalised rotation is replaced
+    by its nearest orthogonal matrix (SVD), then the largest |entry| assigns one voxel axis to one world axis at a time."""
+    rzs = np.asarray(affine, np.float64)[:3, :3]
+    zooms = np.sqrt((rzs ** 2).sum(0))
+    zooms = np.where(zooms == 0, 1.0, zooms)
+    R = rzs / zooms
+    P, _, Qt = np.linalg.svd(R)
+    O = P @ Qt
+    axis, sign = [0, 0, 0], [1, 1, 1]
+    work = np.abs(O)
+    for _ in range(3):
+        w, v = np.unravel_index(np.argmax(work), work.shape)
+        axis[v], sign[v] = int(w), (1 if O[w, v] >= 0 else -1)
+        work[w, :] = -1.0
+        work[:, v] = -1.0
+    cos = [abs(R[axis[v], v]) for v in range(3)]
+    angle = float(np.degrees(np.arccos(min(1.0, min(cos)))))
+    return axis, sign, zooms, angle
+
+
+def to_coronal(data, affine):
+    """-> (array in the coronal frame (a view), its spacing [3] in mm, its voxel-to-world affine, largest axis angle in degrees)"""
+    axis, sign, zooms, angle = orientation(affine)
+    perm, flip = [], []
+    for w, d in FRAME:
+        v = axis.index(w)
+        perm.append(v)
+        flip.append(sign[v] != d)
+    arr = np.transpose(np.asarray(data), perm)
+    F = np.zeros((4, 4))
+    F[3, 3] = 1.0
+    for a, v in enumerate(perm):
+        if flip[a]:
+            arr = np.flip(arr, a)
+            F[v, a], F[v, 3] = -1.0, data.shape[v] - 1.0
+        else:
+            F[v, a] = 1.0
+    return arr, zooms[perm], np.asarray(affine, np.float64) @ F, angle
+
+
+def heart_box(heart):
+    """inclusive voxel index bounds [(lo, hi)] * 3 of the non-zero voxels of a boolean mask"""
+    box = []
+    for a in range(3):
+        nz = np.flatnonzero(np.any(heart, axis=tuple(b for b in range(3) if b != a)))
+        if nz.size == 0:
+            raise ValueError("no MMWHS heart label in the volume")
+        box.append((int(nz[0]), int(nz[-1])))
+    return box
+
+
+def intensity_stats(raw_box):
+    """(p98, mu, sigma) of the raw voxels inside the heart box: linear 98th percentile, then the mean and population standard
+    deviation of min(x, p98), in fp64"""
+    x = np.asarray(raw_box, np.float64)
+    p98 = float(np.percentile(x, 98))
+    clipped = np.minimum(x, p98)
+    mu, sigma = float(clipped.mean()), float(clipped.std())
+    if not sigma > 0:
+        raise ValueError("constant intensity inside the heart box: the volume cannot be z-scored")
+    return p98, mu, sigma
+
+
+def augment_transform(rng):
+    """a 3 x 3 fp64 map from output pixel (r, c, 1) to the un-augmented frame: rotation, per-axis scale, translation (drawn in
+    that order)"""
+    th = np.deg2rad(rng.uniform(-ROTATION_DEG, ROTATION_DEG))
+    s = rng.uniform(SCALE_RANGE[0], SCALE_RANGE[1], 2)
+    t = rng.uniform(-SHIFT_PX, SHIFT_PX, 2)
+    A = np.array([[math.cos(th), -math.sin(th)], [math.sin(th), math.cos(th)]]) @ np.diag(s)
+    T = np.eye(3)
+    T[:2, :2] = A
+    T[:2, 2] = CENTRE + t - A @ np.array([CENTRE, CENTRE])
+    return T
+
+
+def subject_name(image_path):
+    b = os.path.basename(str(image_path))
+    for ext in (".nii.gz", ".nii"):
+        if b.endswith(ext):
+            b = b[:-len(ext)]
+    return b[:-len("_image")] if b.endswith("_image") else b
+
+
+class Subject(object):
+    """One prepared (image, label) pair.  `vol` (fp32) and `cls` (uint8) are the uploaded sub-volume in slice-major order
+    [slice, row, column] of the coronal frame, so a plane's gathers run along contiguous rows.  `D` slices of 256 x 256 pixels of
+    `px` mm; the heart covers slices j_lo .. j_hi (each with both neighbours inside the D)."""
+
+    def __init__(self, image_path, label_path, margin=MARGIN):
+        self.name = subject_name(image_path)
+        im, lb = nifti.load(image_path), nifti.load(label_path)
+        if im.shape != lb.shape or len(im.shape) != 3:
+            raise ValueError("%s: image %s and label %s must be equal-shaped 3-D volumes" % (self.name, im.shape, lb.shape))
+        raw, spacing, self.coronal_affine, angle = to_coronal(im.get_data(), im.get_affine())
+        cls_all, heart, unknown = map_labels(lb.get_data())
+        cls_all = to_coronal(cls_all, im.get_affine())[0]
+        heart = to_coronal(heart, im.get_affine())[0]
+        if unknown:
+            logging.warning("%s: %d label voxels hold values outside the MMWHS set (mapped to background)", self.name, unknown)
+        logging.info("%s: largest angle between a voxel axis and its world axis %.3f degrees", self.name, angle)
+        self.spacing = s = np.asarray(spacing, np.float64)
+        box = heart_box(heart)
+        ext = np.array([(hi - lo + 1) * s[a] for a, (lo, hi) in enumerate(box)])
+        self.centre = c = np.array([(lo + hi) / 2.0 for lo, hi in box])
+        self.px = px = (1.0 + 2.0 * margin) * max(ext[0], ext[1]) / SIZE
+        self.D = D = max(3, int(math.ceil((1.0 + 2.0 * margin) * ext[2] / px)))
+        mid, half = (D - 1) / 2.0, ext[2] / (2.0 * px)
+        self.j_lo, self.j_hi = max(1, int(math.ceil(mid - half))), min(D - 2, int(math.floor(mid + half)))
+        if self.j_lo > self.j_hi:
+            self.j_lo = self.j_hi = min(max(int(round(mid)), 1), D - 2)
+        self.p98, self.mu, self.sigma = intensity_stats(raw[box[0][0]:box[0][1] + 1, box[1][0]:box[1][1] + 1,
+                                                            box[2][0]:box[2][1] + 1])
+        # the sub-volume every sample can reach: REACH_PX in plane, slices 0 .. D-1, one voxel more for the interpolation
+        reach = np.array([REACH_PX * px / s[0], REACH_PX * px / s[1], mid * px / s[2]])
+        self.lo = lo = np.floor(c - reach).astype(np.int64) - 1
+        hi = np.ceil(c + reach).astype(np.int64) + 1
+        idx = [np.arange(lo[a], hi[a] + 1) for a in range(3)]
+        inside = [(i >= 0) & (i < raw.shape[a]) for a, i in enumerate(idx)]
+        clamped = [np.clip(i, 0, raw.shape[a] - 1) for a, i in enumerate(idx)]
+        sub = np.asarray(raw[np.ix_(*clamped)], np.float64)
+        self.vol = np.ascontiguousarray(((np.minimum(sub, self.p98) - self.mu) / self.sigma).astype(np.float32).transpose(2, 0, 1))
+        inside = inside[0][:, None, None] & inside[1][None, :, None] & inside[2][None, None, :]
+        self.cls = np.ascontiguousarray(np.where(inside, cls_all[np.ix_(*clamped)], 0).astype(np.uint8).transpose(2, 0, 1))
+
+    def base(self, j):
+        """3 x 3 fp64 map from un-augmented pixel (r, c, 1) of slice j to this sub-volume's (slice, row, column) coordinates"""
+        s, c, px, lo = self.spacing, self.centre, self.px, self.lo
+        return np.array([[0.0, 0.0, c[2] + (j - (self.D - 1) / 2.0) * px / s[2] - lo[2]],
+                         [px / s[0], 0.0, c[0] - CENTRE * px / s[0] - lo[0]],
+                         [0.0, px / s[1], c[1] - CENTRE * px / s[1] - lo[1]]])
+
+    def matrices(self, slices, T=None, slice_offset=0):
+        """fp32 [len(slices), 3, 3]: base(j) @ T for each slice j (T = None: the identity), composed in fp64 and rounded once;
+        slice_offset shifts the slice coordinate (subjects stacked along the slice axis)"""
+        out = []
+        for j in slices:
+            m = self.base(j) if T is None else self.base(j) @ T
+            m[0, 2] += slice_offset
+            out.append(m)
+        return np.asarray(out, np.float64).astype(np.float32)
+
+    def draw(self, rng, augment=True):
+        """one sample: (slice j, in-plane transform or None); j first, then the augmentation"""
+        j = int(rng.randint(self.j_lo, self.j_hi + 1))
+        return j, (augment_transform(rng) if augment else None)
+
+    def test_affine(self):
+        """voxel-to-world affine of the stored test volume: stored voxel (i, j, k) is training pixel (255 - i, 255 - j) of slice k
+        (the volume is stored flipped along its first two axes; test_eval's flip_correction undoes it)"""
+        s, c, px = self.spacing, self.centre, self.px
+        G = np.array([[px / s[0], 0, 0, c[0] - CENTRE * px / s[0]],
+                      [0, px / s[1], 0, c[1] - CENTRE * px / s[1]],
+                      [0, 0, px / s[2], c[2] - (self.D - 1) / 2.0 * px / s[2]],
+                      [0, 0, 0, 1.0]])
+        S = np.array([[-1.0, 0, 0, SIZE - 1], [0, -1.0, 0, SIZE - 1], [0, 0, 1.0, 0], [0, 0, 0, 1.0]])
+        return self.coronal_affine @ G @ S
+
+
+def stack(subjects):
+    """subjects' sub-volumes stacked along the slice axis, padded to common rows / columns (repeated edge voxels, class 0) ->
+    (vol fp32, cls uint8, slice offset of each subject)"""
+    R = max(s.vol.shape[1] for s in subjects)
+    Cc = max(s.vol.shape[2] for s in subjects)
+    vols, clss, offs, off = [], [], [], 0
+    for s in subjects:
+        pad = ((0, 0), (0, R - s.vol.shape[1]), (0, Cc - s.vol.shape[2]))
+        vols.append(np.pad(s.vol, pad, mode="edge"))
+        clss.append(np.pad(s.cls, pad))
+        offs.append(off)
+        off += s.vol.shape[0]
+    return np.concatenate(vols), np.concatenate(clss), offs
+
+
+def read_pairs(path):
+    """a text file of `image_path label_path` lines -> [(image, label)]; blank lines are skipped"""
+    out = []
+    with open(path) as f:
+        for ln in f:
+            parts = ln.split()
+            if not parts:
+                continue
+            if len(parts) != 2:
+                raise ValueError("%s: expected `image_path label_path`, got %r" % (path, ln.strip()))
+            out.append((parts[0], parts[1]))
+    return out

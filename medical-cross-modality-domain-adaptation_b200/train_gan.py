@@ -64,6 +64,8 @@ def main(phase, argv=None):
     ap.add_argument("--conv-backend", default=None, choices=["auto", "simt", "tc3", "tc1"])
     ap.add_argument("--lists", default="./lists", help="directory of mr_train_list, mr_val_list, ct_train_list, ct_val_list")
     ap.add_argument("--synthetic", action="store_true", help="ignore the list files and train on the synthetic sources")
+    ap.add_argument("--volumes", action="store_true",
+                    help="draw freshly augmented slices on the GPU from the NIfTI pairs of <lists>/{mr,ct}_{train,val}_volumes")
     ap.add_argument("--image-summaries", action="store_true",
                     help="also write the reference's TensorBoard image summaries (prediction, input slice, ground truth) every display step")
     a = ap.parse_args(argv)
@@ -81,8 +83,16 @@ def main(phase, argv=None):
     from .train_segmenter import resolve_lists
     mr_train, mr_val, ct_train, ct_val = resolve_lists(*[os.path.join(a.lists, n) for n in
                                                          ("mr_train_list", "mr_val_list", "ct_train_list", "ct_val_list")], a.synthetic)
+    sources = {}
+    if a.volumes:
+        # each stream keeps the seed of the stream it replaces (adversarial.Trainer.train: 1234 / 4321 / 2234 / 5321 + rank)
+        from .train_segmenter import volume_source
+        rank = parallel.DataParallel().rank
+        for key, name, seed in (("mr_source", "mr_train_volumes", 1234), ("ct_source", "ct_train_volumes", 4321),
+                                ("mr_val_source", "mr_val_volumes", 2234), ("ct_val_source", "ct_val_volumes", 5321)):
+            sources[key] = volume_source(os.path.join(a.lists, name), a.batch_size, seed + rank)
     trainer = drn.Trainer(net, mr_train, mr_val, ct_train, ct_val, num_cls=num_cls, batch_size=a.batch_size,
-                          opt_kwargs=dict(opt_kwargs), train_config=tc)
+                          opt_kwargs=dict(opt_kwargs), train_config=tc, **sources)
     print("Now start training...")
     return trainer.train(output_path=out, restored_path=out, training_iters=a.training_iters or tc["training_iters"],
                          epochs=a.epochs or tc["epochs"], dropout=a.keep_prob, image_summaries=a.image_summaries)

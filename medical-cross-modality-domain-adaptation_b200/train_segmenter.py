@@ -43,6 +43,15 @@ def resolve_lists(*fids_and_flag):
     return out
 
 
+def volume_source(pairs_file, batch_size, seed):
+    """data.VolumeSource over the `image label` pairs of a list file"""
+    from .data import VolumeSource
+    from .preprocess import read_pairs
+    pairs = read_pairs(pairs_file)
+    logging.info("%s: %d volume pairs" % (pairs_file, len(pairs)))
+    return VolumeSource(pairs, batch_size, seed)
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch-size", type=int, default=batch_size)
@@ -54,6 +63,9 @@ def main(argv=None):
     ap.add_argument("--train-list", default=train_fid)
     ap.add_argument("--val-list", default=val_fid)
     ap.add_argument("--synthetic", action="store_true", help="ignore the list files and train on the synthetic source")
+    ap.add_argument("--train-volumes", default=None,
+                    help="file of `image label` NIfTI pairs: draw freshly augmented training slices from these volumes on the GPU")
+    ap.add_argument("--val-volumes", default=None, help="file of `image label` NIfTI pairs: validation slices from these volumes")
     ap.add_argument("--image-summaries", action="store_true",
                     help="also write the reference's TensorBoard image summaries (prediction, input slice, ground truth) every display step")
     a = ap.parse_args(argv)
@@ -64,8 +76,11 @@ def main(argv=None):
     net = drn.Full_DRN(channels=3, n_class=num_cls, batch_size=a.batch_size, cost_kwargs=dict(cost_kwargs))
     print("Network has been built ...")
     train_list, val_list = resolve_lists(a.train_list, a.val_list, a.synthetic)
+    # VolumeSource streams take the seeds of the streams they replace (source_segmenter.Trainer.train: 1234 / 4321 + rank)
+    sources = {k: volume_source(path, a.batch_size, seed + parallel.DataParallel().rank) for k, path, seed in
+               (("source", a.train_volumes, 1234), ("val_source", a.val_volumes, 4321)) if path}
     trainer = drn.Trainer(net, train_list=train_list, val_list=val_list, num_cls=num_cls, batch_size=a.batch_size, opt_kwargs=dict(opt_kwargs),
-                          checkpoint_space=checkpoint_space, optimizer=optimizer, lr_update_flag=False)
+                          checkpoint_space=checkpoint_space, optimizer=optimizer, lr_update_flag=False, **sources)
     print("Now start training...")
     return trainer.train(output_path=a.output_path, restored_path=a.output_path, training_iters=a.training_iters,
                          epochs=a.epochs, restore=restore, dropout=a.keep_prob, image_summaries=a.image_summaries)
