@@ -343,6 +343,22 @@ int pnp_surface_distance(const uint8_t* pred, const uint8_t* gt, int n0, int n1,
 int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W, int C,
                         float* img, long long* lab, int label_planes, void* stream);
 
+/* ---- native-grid labels: a prepared-grid prediction sampled back onto the scan's own voxels (resample.cu) ------------------------
+ * scores: fp32 C-order [n0][n1][n2][C] class scores on the prepared grid (slice, row, column; C fastest), device.  map: 12 fp32
+ * (device) taking native voxel (i, j, k) to the prepared coordinate
+ *   u_a = ((m[4a] * i + m[4a+1] * j) + m[4a+2] * k) + m[4a+3],   a = 0, 1, 2,
+ * each product and each sum rounded separately in fp32 (no FMA contraction).  For every native voxel of the C-order [m0][m1][m2]
+ * grid (the order nifti.load(...).get_data() returns):
+ *   out (uint8): 0 when any u_a is outside [-0.5, n_a - 0.5) or NaN; otherwise the argmax over c (the lowest index wins a tie) of
+ *     the trilinear score of class c, with pnp_resample_planes' clamp, taps and lerp order (axis 2, then 1, then 0).
+ *   cm (int64 [C][C], device, optional with gt): cm[gt][out] counted over every voxel, gt uint8 [m0][m1][m2] on the device;
+ *     ground-truth labels >= C count as background.  The call zeroes cm first; integer counts make repeated calls bit-identical.
+ * gt and cm are both NULL or both given.  NULL scores / map / out, only one of gt / cm, or a non-positive size are
+ * PNP_ERR_BAD_ARG; C outside [2, 8], a dimension above PNP_RS_MAX_DIM, or n0*n1*n2*C or m0*m1*m2 >= 2^31 are
+ * PNP_ERR_UNSUPPORTED.  On any error nothing is launched and the outputs are untouched. */
+int pnp_native_labels(const float* scores, int n0, int n1, int n2, int C, const float* map, int m0, int m1, int m2, uint8_t* out,
+                      const uint8_t* gt, long long* cm, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -104,6 +104,7 @@ SIGNATURES = {
     "pnp_surface_distance_workspace": [c_int, c_int, c_int, c_int, P],
     "pnp_surface_distance": [P, P, c_int, c_int, c_int, c_int, P, P, c_ll, P, P],
     "pnp_resample_planes": [P, P, c_int, c_int, c_int, P, c_int, c_int, c_int, c_int, P, P, c_int, P],
+    "pnp_native_labels": [P, c_int, c_int, c_int, c_int, P, c_int, c_int, c_int, P, P, P, P],
 }
 
 for _name, _args in SIGNATURES.items():

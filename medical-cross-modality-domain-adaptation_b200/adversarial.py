@@ -511,16 +511,20 @@ class Trainer(object):
                 f.write(json.dumps(dict(step=int(step), **scalars)) + "\n")
         return scalars
 
+    def _ct_logits(self, x):
+        """the test protocol's forward: inference-mode adapted CT stream (keep_prob 1, every BN switch off -- the feed of
+        adversarial.py:1036-1038), x [B, 256, 256, 3] on the device -> logits [B, 256, 256, C]"""
+        return self.net.segment(x, "ct", 1.0, front_bn=False, joint_bn=False)["logits"]
+
     def _predict_ct(self, vol, sl):
-        """one forward call of the test protocol: inference-mode adapted CT stream (keep_prob 1, every BN switch off -- the feed of
-        adversarial.py:1036-1038) -> (argmax labels, confusion counts [label, prediction]) on the host"""
+        """one forward call of the test protocol (_ct_logits) -> (argmax labels, confusion counts [label, prediction]) on the host"""
         from .lib import _label_decomp
         nc = self.num_cls or self.net.n_class
         dev = rt.device()
         x = torch.from_numpy(np.ascontiguousarray(vol, np.float32)).to(dev)
         y = _label_decomp(nc, torch.from_numpy(np.ascontiguousarray(sl, np.int64)).to(dev))
         with torch.no_grad():
-            logits = self.net.segment(x, "ct", 1.0, front_bn=False, joint_bn=False)["logits"]
+            logits = self._ct_logits(x)
             cm = F.confusion_counts(logits, y)
             pred = logits.argmax(3)
         return pred.cpu().numpy(), cm.cpu().numpy()
@@ -556,6 +560,13 @@ class Trainer(object):
             evaluation.surface_metric_stddev(res[2], nc)
             evaluation.write_surface_csv(os.path.join(output_path, "surface.csv"), res[2], nc)
         return out
+
+    def test_native(self, pairs, output_path):
+        """every raw (image, label) pair segmented on its own grid by the adapted CT stream (native.run): writes
+        <output_path>/native_pred/<name>_label.nii.gz and native.csv, prints per-organ Dice and ASSD / HD in mm -> per-subject
+        results"""
+        from . import native
+        return native.run(self._ct_logits, pairs, output_path, self.net.batch_size, self.num_cls or self.net.n_class)
 
     def sample_metric_stddev(self, sample_eval_list):
         """adversarial.py:1054-1084"""

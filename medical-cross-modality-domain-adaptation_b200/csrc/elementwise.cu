@@ -1597,4 +1597,4 @@ extern "C" const char* pnp_error_string(int code) {
   }
 }
 
-extern "C" int pnp_version(void) { return 103; }
+extern "C" int pnp_version(void) { return 104; }

@@ -2,7 +2,8 @@
 // augmented coronal slice of a batch -- images by trilinear interpolation of the z-scored intensities, labels by the nearest voxel
 // of the class-id volume -- straight into the trainers' NHWC layout, so a trainer can draw fresh augmentations every step
 // without record files or a host-to-device image copy.  A grid-stride gather: the writes are coalesced along the NHWC index,
-// the reads follow the sampled coordinates.
+// the reads follow the sampled coordinates.  The way back (native.py): pnp_native_labels samples the class scores of the prepared
+// grid at every voxel of the subject's native grid with the same taps and lerps, and labels it by their argmax.
 #include "common.cuh"
 #include "../../include/pnp_b200.h"
 
@@ -24,10 +25,13 @@ __device__ __forceinline__ void axis_taps(float u, int n, int& i0, int& i1, floa
   f = __fsub_rn(x, fl);
 }
 
-// nearest voxel floor(u + 0.5) (ties round up), -1 outside [-0.5, n - 0.5) or for a NaN coordinate.  n <= 2^23 keeps n - 0.5
-// exact; the min() only guards the index.
+// u inside [-0.5, n - 0.5), false for a NaN coordinate.  n <= 2^23 keeps n - 0.5 exact.
+__device__ __forceinline__ bool axis_inside(float u, int n) { return u >= -0.5f && u < __fsub_rn((float)n, 0.5f); }
+
+// nearest voxel floor(u + 0.5) (ties round up), -1 outside [-0.5, n - 0.5) or for a NaN coordinate; the min() only guards the
+// index.
 __device__ __forceinline__ int axis_nearest(float u, int n) {
-  if (!(u >= -0.5f && u < __fsub_rn((float)n, 0.5f))) return -1;
+  if (!axis_inside(u, n)) return -1;
   return min((int)floorf(__fadd_rn(u, 0.5f)), n - 1);
 }
 
@@ -75,6 +79,68 @@ resample_planes_kernel(const float* __restrict__ vol, const uint8_t* __restrict_
   }
 }
 
+// Native voxel q = (i m1 + j) m2 + k: trilinear class scores at its prepared-grid coordinate, first-max argmax, and with gt the
+// (truth, prediction) pair in a per-CTA histogram flushed by one global atomic per non-zero bin.
+__global__ void __launch_bounds__(256)
+native_labels_kernel(const float* __restrict__ scores, int n0, int n1, int n2, int C, const float* __restrict__ map, int m1, int m2,
+                     long long total, uint8_t* __restrict__ out, const uint8_t* __restrict__ gt, long long* __restrict__ cm) {
+  __shared__ unsigned int hist[64];
+  pnp_pdl_enter();
+  if (cm) {
+    if (threadIdx.x < 64) hist[threadIdx.x] = 0u;
+    __syncthreads();
+  }
+  float m[12];
+#pragma unroll
+  for (int t = 0; t < 12; ++t) m[t] = __ldg(map + t);
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const unsigned q = (unsigned)i;
+    const unsigned row = q / (unsigned)m2;
+    const float fk = (float)(q - row * (unsigned)m2), fj = (float)(row % (unsigned)m1), fi = (float)(row / (unsigned)m1);
+    float u[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+      u[a] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[4 * a], fi), __fmul_rn(m[4 * a + 1], fj)), __fmul_rn(m[4 * a + 2], fk)),
+                       m[4 * a + 3]);
+    int best = 0;
+    if (axis_inside(u[0], n0) && axis_inside(u[1], n1) && axis_inside(u[2], n2)) {
+      int a0, b0, a1, b1, a2, b2;
+      float f0, f1, f2;
+      axis_taps(u[0], n0, a0, b0, f0);
+      axis_taps(u[1], n1, a1, b1, f1);
+      axis_taps(u[2], n2, a2, b2, f2);
+      const float* p00 = scores + (long long)((a0 * n1 + a1) * n2) * C;
+      const float* p01 = scores + (long long)((a0 * n1 + b1) * n2) * C;
+      const float* p10 = scores + (long long)((b0 * n1 + a1) * n2) * C;
+      const float* p11 = scores + (long long)((b0 * n1 + b1) * n2) * C;
+      const int o0 = a2 * C, o1 = b2 * C;
+      float top = 0.f;
+      for (int c = 0; c < C; ++c) {
+        const float v00 = lerp_rn(__ldg(p00 + o0 + c), __ldg(p00 + o1 + c), f2);
+        const float v01 = lerp_rn(__ldg(p01 + o0 + c), __ldg(p01 + o1 + c), f2);
+        const float v10 = lerp_rn(__ldg(p10 + o0 + c), __ldg(p10 + o1 + c), f2);
+        const float v11 = lerp_rn(__ldg(p11 + o0 + c), __ldg(p11 + o1 + c), f2);
+        const float v = lerp_rn(lerp_rn(v00, v01, f1), lerp_rn(v10, v11, f1), f0);
+        if (c == 0 || v > top) {       // strictly greater: the lowest index wins a tie
+          top = v;
+          best = c;
+        }
+      }
+    }
+    out[q] = (uint8_t)best;
+    if (cm) {
+      int g = __ldg(gt + q);
+      if (g >= C) g = 0;
+      atomicAdd(&hist[g * C + best], 1u);
+    }
+  }
+  if (cm) {
+    __syncthreads();
+    if (threadIdx.x < C * C && hist[threadIdx.x])
+      atomicAdd((unsigned long long*)cm + threadIdx.x, (unsigned long long)hist[threadIdx.x]);
+  }
+}
+
 // a product of positive ints below 2^31 (each factor is, so no partial product overflows)
 bool count_below_2_31(std::initializer_list<int> dims) {
   long long n = 1;
@@ -100,5 +166,21 @@ extern "C" int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0,
   const long long total = (long long)B * H * W * Cw;
   PNP_CUDA(pnp_launch(resample_planes_kernel, grid_for(total, 256 * 4), 256, 0, (cudaStream_t)stream, vol, cls, n0, n1, n2, mats, H, W,
                       C, Cw, total, img, lab, label_planes));
+  return PNP_OK;
+}
+
+extern "C" int pnp_native_labels(const float* scores, int n0, int n1, int n2, int C, const float* map, int m0, int m1, int m2,
+                                 uint8_t* out, const uint8_t* gt, long long* cm, void* stream) {
+  if (!scores || !map || !out || (!gt) != (!cm) || n0 <= 0 || n1 <= 0 || n2 <= 0 || m0 <= 0 || m1 <= 0 || m2 <= 0)
+    return PNP_ERR_BAD_ARG;
+  if (C < 2 || C > 8) return PNP_ERR_UNSUPPORTED;
+  if (n0 > PNP_RS_MAX_DIM || n1 > PNP_RS_MAX_DIM || n2 > PNP_RS_MAX_DIM || m0 > PNP_RS_MAX_DIM || m1 > PNP_RS_MAX_DIM ||
+      m2 > PNP_RS_MAX_DIM)
+    return PNP_ERR_UNSUPPORTED;
+  if (!count_below_2_31({n0, n1, n2, C}) || !count_below_2_31({m0, m1, m2})) return PNP_ERR_UNSUPPORTED;
+  const long long total = (long long)m0 * m1 * m2;
+  if (cm) PNP_CUDA(cudaMemsetAsync(cm, 0, sizeof(long long) * C * C, (cudaStream_t)stream));
+  PNP_CUDA(pnp_launch(native_labels_kernel, grid_for(total, 256 * 4), 256, 0, (cudaStream_t)stream, scores, n0, n1, n2, C, map, m1,
+                      m2, total, out, gt, cm));
   return PNP_OK;
 }

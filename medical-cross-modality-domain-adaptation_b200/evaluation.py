@@ -115,21 +115,21 @@ def _organ_names(num_cls):
     return [names.get(c, "class_%d" % c) for c in range(num_cls)]
 
 
-def surface_metric_stddev(sample_surface_list, num_cls):
+def surface_metric_stddev(sample_surface_list, num_cls, units="voxel units"):
     """Per-organ spread and mean of ASSD and HD over subjects, printed in the form of sample_metric_stddev's lines.  Subjects where
     the organ is absent from the prediction or the ground truth (NaN) are left out and counted.  Returns (mean ASSD [num_cls],
-    mean HD [num_cls]), NaN where no subject has the organ in both volumes."""
+    mean HD [num_cls]), NaN where no subject has the organ in both volumes.  `units` names the distances' unit in the headings."""
     names = _organ_names(num_cls)
     stats = {}
     for key in ("assd", "hd"):
         mat = np.array([s[key] for s in sample_surface_list], np.float64).reshape(len(sample_surface_list), num_cls)
         stats[key] = [mat[~np.isnan(mat[:, c]), c] for c in range(num_cls)]
-    print("------- surface distances over subjects (voxel units) ---- ")
+    print("------- surface distances over subjects (%s) ---- " % units)
     for c in range(1, num_cls):
         print("organ: %s" % names[c])
         print("assd_stddev: %s" % (np.std(stats["assd"][c]) if len(stats["assd"][c]) else np.nan))
         print("hd_stddev: %s" % (np.std(stats["hd"][c]) if len(stats["hd"][c]) else np.nan))
-    print("------- surface distances over subjects (voxel units) ----  ")
+    print("------- surface distances over subjects (%s) ----  " % units)
     mean = {k: np.full(num_cls, np.nan) for k in ("assd", "hd")}
     for c in range(1, num_cls):
         print("organ: %s" % names[c])

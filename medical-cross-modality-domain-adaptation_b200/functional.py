@@ -1093,6 +1093,26 @@ def resample_planes(vol, cls, mats, H, W, image=True, label_planes=1, img=None, 
     return (img if image else None), (lab if label_planes else None)
 
 
+def native_labels(scores, vmap, shape, gt=None, out=None):
+    """A prepared-grid prediction sampled back onto a native grid in one pnp_native_labels launch (include/pnp_b200.h,
+    "native-grid labels").  `scores` fp32 [n0, n1, n2, C] on the device, `vmap` fp32 [12] (device) from native voxel to prepared
+    coordinate, `shape` the native (m0, m1, m2).  Returns (labels uint8 [m0, m1, m2], confusion counts int64 [C, C] (rows =
+    truth) or None); `gt` uint8 [m0, m1, m2] on the device asks for the counts, `out` may be given to write into."""
+    scores, vmap = scores.contiguous(), vmap.contiguous()
+    n0, n1, n2, C = scores.shape
+    m0, m1, m2 = (int(s) for s in shape)
+    if out is None:
+        out = torch.empty(m0, m1, m2, dtype=torch.uint8, device=scores.device)
+    cm = None
+    if gt is not None:
+        gt = gt.contiguous()
+        if tuple(gt.shape) != (m0, m1, m2) or gt.dtype != torch.uint8:
+            raise ValueError("native_labels: gt must be uint8 %s, got %s %s" % ((m0, m1, m2), tuple(gt.shape), gt.dtype))
+        cm = torch.empty(C, C, dtype=torch.int64, device=scores.device)
+    call("pnp_native_labels", ptr(scores), n0, n1, n2, C, ptr(vmap), m0, m1, m2, ptr(out), ptr(gt), ptr(cm), rt.stream())
+    return out, cm
+
+
 def confusion_counts(logits, y):
     """[C,C] int64 confusion matrix (rows = truth) of argmax(logits) vs one-hot y (lib.py:96-110)."""
     logits, y = logits.contiguous(), y.contiguous()

@@ -78,23 +78,32 @@ def orientation(affine):
     return axis, sign, zooms, angle
 
 
-def to_coronal(data, affine):
-    """-> (array in the coronal frame (a view), its spacing [3] in mm, its voxel-to-world affine, largest axis angle in degrees)"""
+def coronal_frame(affine, shape):
+    """the coronal frame of a volume of `shape` stored with `affine` -> (perm, flip, F, zooms, angle): coronal axis a is voxel axis
+    perm[a], reversed where flip[a]; F (4 x 4) maps coronal voxel to stored voxel; zooms and angle as orientation() returns them"""
     axis, sign, zooms, angle = orientation(affine)
     perm, flip = [], []
     for w, d in FRAME:
         v = axis.index(w)
         perm.append(v)
         flip.append(sign[v] != d)
-    arr = np.transpose(np.asarray(data), perm)
     F = np.zeros((4, 4))
     F[3, 3] = 1.0
     for a, v in enumerate(perm):
         if flip[a]:
-            arr = np.flip(arr, a)
-            F[v, a], F[v, 3] = -1.0, data.shape[v] - 1.0
+            F[v, a], F[v, 3] = -1.0, shape[v] - 1.0
         else:
             F[v, a] = 1.0
+    return perm, flip, F, zooms, angle
+
+
+def to_coronal(data, affine):
+    """-> (array in the coronal frame (a view), its spacing [3] in mm, its voxel-to-world affine, largest axis angle in degrees)"""
+    perm, flip, F, zooms, angle = coronal_frame(affine, np.shape(data))
+    arr = np.transpose(np.asarray(data), perm)
+    for a in range(3):
+        if flip[a]:
+            arr = np.flip(arr, a)
     return arr, zooms[perm], np.asarray(affine, np.float64) @ F, angle
 
 
@@ -153,6 +162,10 @@ class Subject(object):
         if im.shape != lb.shape or len(im.shape) != 3:
             raise ValueError("%s: image %s and label %s must be equal-shaped 3-D volumes" % (self.name, im.shape, lb.shape))
         raw, spacing, self.coronal_affine, angle = to_coronal(im.get_data(), im.get_affine())
+        # the native grid, for predictions written back onto it (native.py): shape, affine, and coronal voxel -> native voxel
+        self.native_shape = tuple(int(n) for n in im.shape)
+        self.native_affine = np.asarray(im.get_affine(), np.float64)
+        self.frame = coronal_frame(self.native_affine, self.native_shape)[2]
         cls_all, heart, unknown = map_labels(lb.get_data())
         cls_all = to_coronal(cls_all, im.get_affine())[0]
         heart = to_coronal(heart, im.get_affine())[0]

@@ -394,14 +394,18 @@ class Trainer(object):
         return {"loss": self.net.cost_value(wce, dice), "dice_eval": float(d), "dice_arr": [float(a) for a in arr]}
 
     # ---- test protocol on NIfTI subjects (source_segmenter.py:572-675) -----------------------------------------------
+    def _logits(self, x):
+        """the test protocol's forward: keep_prob 1, main_bn / adapt_bn off (the feed of source_segmenter.py:615-617), x [B, 256,
+        256, 3] on the device -> logits [B, 256, 256, C]"""
+        return self.net.forward(x, keep_prob=1.0, main_bn=False, adapt_bn=False)
+
     def _predict(self, vol, sl):
-        """one forward call of the test protocol: keep_prob 1, main_bn / adapt_bn off (the feed of source_segmenter.py:615-617)
-        -> (argmax labels, confusion counts [label, prediction]) on the host"""
+        """one forward call of the test protocol (_logits) -> (argmax labels, confusion counts [label, prediction]) on the host"""
         dev = rt.device()
         x = torch.from_numpy(np.ascontiguousarray(vol, np.float32)).to(dev)
         y = _label_decomp(self.num_cls, torch.from_numpy(np.ascontiguousarray(sl, np.int64)).to(dev))
         with torch.no_grad():
-            logits = self.net.forward(x, keep_prob=1.0, main_bn=False, adapt_bn=False)
+            logits = self._logits(x)
             cm = self.net.confusion_matrix(logits, y)
             pred = logits.argmax(3)
         return pred.cpu().numpy(), cm.cpu().numpy()
@@ -430,6 +434,12 @@ class Trainer(object):
             evaluation.surface_metric_stddev(res[2], self.num_cls)
             evaluation.write_surface_csv(os.path.join(output_path, "surface.csv"), res[2], self.num_cls)
         return out
+
+    def test_native(self, pairs, output_path):
+        """every raw (image, label) pair segmented on its own grid (native.run): writes <output_path>/native_pred/<name>_label.nii.gz
+        and native.csv, prints per-organ Dice and ASSD / HD in mm -> per-subject results"""
+        from . import native
+        return native.run(self._logits, pairs, output_path, self.net.batch_size, self.num_cls)
 
     def sample_metric_stddev(self, sample_eval_list):
         """source_segmenter.py:634-664"""
