@@ -117,6 +117,11 @@ lib.pnp_version.restype = c_int
 lib.pnp_tc_available.restype = c_int
 lib.pnp_tc_last_config.argtypes = [P, P, P]
 lib.pnp_tc_last_config.restype = c_int
+# residency of the wgmma convolutions (conv_tc.cu; test and profiling aids outside the C-ABI header)
+lib.pnp_tc_last_residency.argtypes = [P, P]
+lib.pnp_tc_last_residency.restype = c_int
+lib.pnp_tc_set_residency_cap.argtypes = [c_int]
+lib.pnp_tc_set_residency_cap.restype = c_int
 
 # launch counter: bench.py reports how many of OUR kernels ran inside the timed region
 launch_count = 0

@@ -19,7 +19,8 @@
 // NTERMS == 1 is the plain bf16 path of BASELINE config 5.
 //
 // Warp roles (288 threads): warps 0..7 = two consumer warpgroups (accumulator rows 0..63 and 64..127: one m64nNk16 wgmma
-// each per K step), warp 8 = TMA producer (one lane).
+// each per K step), warp 8 = TMA producer (one lane).  Tiles of at most 64 columns run two CTAs per SM (96 registers per
+// thread, half the shared-memory ring each), the 128-column tiles one.
 #include <cuda.h>
 #include <cstdio>
 #include <cstdlib>
@@ -291,13 +292,20 @@ __device__ __forceinline__ void kblock_of(const TcArgs& a, const TileCoord& tc, 
   tap = tc.tap_begin + tl;
 }
 
-template <int BLOCK_N, int NTERMS, int BK>
+// CTAs resident per SM: two for the accumulators of at most 64 columns (32 fp32 registers per thread), so that one CTA's
+// epilogue runs while the other issues MMAs; the 128-column tiles need more than the 96 registers per thread two CTAs of
+// 288 threads can have (registers are allocated per 16K-register SM sub-partition, and 18 warps put five on one), and stay
+// at one
+constexpr int tc_ctas_per_sm(int block_n) { return block_n <= 64 ? 2 : 1; }
+
+template <int BLOCK_N, int NTERMS, int BK, int CTAS_PER_SM>
 struct TcCfg {
   static constexpr int A_TILE_BYTES = BLOCK_M * BK * 2;
   static constexpr int B_TILE_BYTES = BLOCK_N * BK * 2;
   static constexpr int NPLANES = (NTERMS == 1) ? 1 : 2;
   static constexpr int STAGE_BYTES = NPLANES * (A_TILE_BYTES + B_TILE_BYTES);
-  static constexpr int STAGES_RAW = (200 * 1024) / STAGE_BYTES;
+  // the ~200 KB ring budget of an SM is shared by its resident CTAs
+  static constexpr int STAGES_RAW = (200 * 1024 / CTAS_PER_SM) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
   // fp64 BN partial sums of the current n-tile, one [sum | sumsq][BLOCK_N] row per consumer warp (16 KB at BLOCK_N = 128)
   static constexpr int STAT_BYTES = CONSUMER_WARPS * 2 * BLOCK_N * 8;
@@ -305,20 +313,23 @@ struct TcCfg {
   static_assert(STAGES >= 2, "pipeline needs two stages");
   // the ring is sized before the statistics rows: they must fit beside it, never cost it a stage
   static_assert(SMEM_BYTES <= 227 * 1024, "H100 allows 227 KB of shared memory per block");
+  // every resident CTA also takes 1 KB of shared memory the system reserves, out of the SM's 228 KB
+  static_assert(CTAS_PER_SM * (SMEM_BYTES + 1024) <= 228 * 1024, "the resident CTAs must fit in one SM's shared memory");
 };
 
 // 32-bit word k (0..3, may differ per lane) of a Philox block
 __device__ __forceinline__ uint32_t word_of(const uint4& r, int k) { return k == 0 ? r.x : k == 1 ? r.y : k == 2 ? r.z : r.w; }
 
-template <int BLOCK_N, int NTERMS, int BK>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+template <int BLOCK_N, int NTERMS, int BK, int CTAS_PER_SM>
+__global__ void __launch_bounds__(TC_THREADS, CTAS_PER_SM)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
                float* __restrict__ out, TcArgs a) {
   pnp_pdl_trigger();      // the wait comes after the prologue (barriers, tensor-map prefetch touch no predecessor data)
-  // PERSISTENT: one CTA per SM walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...; the smem ring and its phases run
-  // across tile boundaries, so the producer prefetches the next tile's operands while the consumers run the epilogue.
-  using Cfg = TcCfg<BLOCK_N, NTERMS, BK>;
+  // PERSISTENT: CTAS_PER_SM CTAs per SM walk tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...; the smem ring and its phases
+  // run across tile boundaries, so the producer prefetches the next tile's operands while the consumers run the epilogue, and
+  // with two CTAs on an SM the other CTA's MMAs run during it too.
+  using Cfg = TcCfg<BLOCK_N, NTERMS, BK, CTAS_PER_SM>;
   constexpr int A_TILE_BYTES = Cfg::A_TILE_BYTES;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int ACC = BLOCK_N / 2;                   // fp32 accumulator registers per thread (m64 x BLOCK_N per warpgroup)
@@ -391,6 +402,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   const bool drop_on = a.drop.seed_ptr != nullptr;
   unsigned long long seed = 0ull;
   if (drop_on) seed = *a.drop.seed_ptr;
+  // At two CTAs per SM a thread has 96 registers, a third of them the accumulator.  The empty asm statements guarded by
+  // SHORT_LIVES below keep the compiler from holding values over the K loop or the epilogue's loops that it can form again
+  // cheaply; the one-CTA instantiations have the registers to spare and are compiled as before.
+  constexpr bool SHORT_LIVES = CTAS_PER_SM > 1;
   // BN partial statistics: warp-reduced in fp32, then summed in fp64 over every tile of this CTA that shares an n-tile, in the
   // warp's own shared-memory row (one writer per slot: plain adds, no shared-memory atomics, which sm_90 runs as CAS loops on
   // fp64).  When the n-tile changes (and at the end) the eight rows are summed in a fixed order and each column takes one fp64
@@ -415,18 +430,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   int stage = 0;
   uint32_t phase = 0;
   for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
-    const TileCoord tc = decode_tile<BLOCK_N>(a, t, n_tiles);
-    const int n0 = tc.n0;
-    if (bn_on && n0 != stat_n0) {
+    const TileCoord tk = decode_tile<BLOCK_N>(a, t, n_tiles);
+    if (bn_on && tk.n0 != stat_n0) {
       if (stat_n0 >= 0) flush_stats();
-      stat_n0 = n0;
+      stat_n0 = tk.n0;
     }
-    if (tc.kb_count == 0) {
+    const int kb_count = tk.kb_count;
+    if (kb_count == 0) {
 #pragma unroll
       for (int i = 0; i < ACC; ++i) acc[i] = 0.f;
     }
     int prev = -1;
-    for (int kb = 0; kb < tc.kb_count; ++kb) {
+    for (int kb = 0; kb < kb_count; ++kb) {
       mbar_wait(smem_u32(&bars[stage]), phase);
       wgmma_fence();
       const uint32_t st = smem_u32(smem + stage * Cfg::STAGE_BYTES);
@@ -466,6 +481,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
       if (lane == 0) mbar_arrive(smem_u32(&bars[STAGES + prev]));
     }
 
+    // the tile's coordinates: with SHORT_LIVES decoded again rather than held over the K loop (the asm hides that t_ep is
+    // the t decoded above); otherwise the compiler merges this with the decode above
+    int t_ep = t;
+    if constexpr (SHORT_LIVES) asm volatile("" : "+r"(t_ep));
+    const TileCoord tc = decode_tile<BLOCK_N>(a, t_ep, n_tiles);
+    const int n0 = tc.n0;
     // the rows' coordinates are derived per tile rather than kept live across the K loop
     long long pix[2];
     bool valid[2];
@@ -546,10 +567,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (!valid[h]) continue;
+        // with SHORT_LIVES the row's addresses are formed per column group: hoisted out of the unrolled loop, the 64-bit row
+        // pointers of y, its planes and the skip would take a dozen registers through the whole column loop
+        long long p = pix[h];
+        if constexpr (SHORT_LIVES) asm volatile("" : "+l"(p));
         float2 o = make_float2(v[h][0], v[h][1]);
         if (a.ep_scale != nullptr) { o.x = fmaf(o.x, sc.x, sh.x); o.y = fmaf(o.y, sc.y, sh.y); }
         if (skip_on) {
-          const float2 sk = __ldg(reinterpret_cast<const float2*>(a.ep_skip + pix[h] * a.ep_skip_c - a.ep_skip_off + ch));
+          const float2 sk = __ldg(reinterpret_cast<const float2*>(a.ep_skip + p * a.ep_skip_c - a.ep_skip_off + ch));
           o.x += sk.x; o.y += sk.y;
         }
         // positive subnormals go to +0, as in elementwise.cu act_fwd: the hi plane of y then carries the sign of y exactly
@@ -561,7 +586,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
           o.x = o.x >= kMinNormal ? o.x : (o.x > 0.f ? 0.f : 0.2f * o.x);
           o.y = o.y >= kMinNormal ? o.y : (o.y > 0.f ? 0.f : 0.2f * o.y);
         }
-        const long long e0 = pix[h] * a.Cout + ch;   // flat element index of this thread's pair
+        const long long e0 = p * a.Cout + ch;        // flat element index of this thread's pair
         if (out != nullptr) {
           float2* dst = reinterpret_cast<float2*>(out + e0);
           if (a.ksplit > 1) {
@@ -933,19 +958,29 @@ int sm_count() {
   return num_sms;
 }
 
+// {CTAs per SM, grid size} of the most recent conv launch, and the largest residency a launch may use (profiling aids)
+int g_last_residency[2] = {0, 0};
+int g_residency_cap = 2;
+
 template <int BLOCK_N, int NTERMS, int BK>
 int launch_tc(const CUtensorMap& ma_hi, const CUtensorMap& ma_lo, const CUtensorMap& mb_hi, const CUtensorMap& mb_lo,
               float* y, const TcArgs& a, cudaStream_t s) {
-  using Cfg = TcCfg<BLOCK_N, NTERMS, BK>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PNP_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, NTERMS, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    attr_set = true;
+  constexpr int CTAS = tc_ctas_per_sm(BLOCK_N);
+  using Cfg = TcCfg<BLOCK_N, NTERMS, BK, CTAS>;
+  auto kernel = conv_tc_kernel<BLOCK_N, NTERMS, BK, CTAS>;
+  static int resident = 0;            // CTAs per SM the device actually fits, checked on the first launch
+  if (resident == 0) {
+    PNP_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    int fit = 0;
+    PNP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, kernel, TC_THREADS, Cfg::SMEM_BYTES));
+    resident = fit >= CTAS ? CTAS : 1;      // a device that fits fewer runs the same kernel at one CTA per SM
   }
-  const int num_sms = sm_count();
+  const int ctas = resident < g_residency_cap ? resident : g_residency_cap;
+  const long long slots = (long long)ctas * sm_count();
   const long long tiles = a.total_tiles;
-  dim3 grid((unsigned)(tiles < num_sms ? tiles : num_sms));     // persistent: one CTA per SM walks the tile list
-  pnp_launch(conv_tc_kernel<BLOCK_N, NTERMS, BK>, grid, TC_THREADS, Cfg::SMEM_BYTES, s, ma_hi, ma_lo, mb_hi, mb_lo, y, a);
+  dim3 grid((unsigned)(tiles < slots ? tiles : slots));     // persistent: the resident CTAs walk the tile list
+  g_last_residency[0] = ctas; g_last_residency[1] = (int)grid.x;
+  pnp_launch(kernel, grid, TC_THREADS, Cfg::SMEM_BYTES, s, ma_hi, ma_lo, mb_hi, mb_lo, y, a);
   PNP_LAUNCH_CHECK();
   return PNP_OK;
 }
@@ -1086,6 +1121,21 @@ extern "C" int pnp_tc_last_config(int* block_n, int* block_k, int* ksplit) {
   if (block_k) *block_k = g_last_cfg[1];
   if (ksplit) *ksplit = g_last_cfg[2];
   return PNP_OK;
+}
+
+// Residency of the wgmma forward / data-gradient launches, for tests and profiling (not part of the C-ABI header):
+// pnp_tc_last_residency reports the CTAs per SM and the grid of the most recent launch; pnp_tc_set_residency_cap(1) runs
+// every later launch at one CTA per SM (2 restores the default) and returns the previous cap.
+extern "C" int pnp_tc_last_residency(int* ctas_per_sm, int* grid) {
+  if (ctas_per_sm) *ctas_per_sm = g_last_residency[0];
+  if (grid) *grid = g_last_residency[1];
+  return PNP_OK;
+}
+
+extern "C" int pnp_tc_set_residency_cap(int cap) {
+  const int prev = g_residency_cap;
+  if (cap == 1 || cap == 2) g_residency_cap = cap;
+  return prev;
 }
 
 extern "C" int pnp_tc_available(void) {
