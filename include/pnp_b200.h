@@ -320,6 +320,25 @@ int pnp_surface_distance_workspace(int n0, int n1, int n2, int C, long long* byt
 int pnp_surface_distance(const uint8_t* pred, const uint8_t* gt, int n0, int n1, int n2, int C, const double* spacing /* host, 3 */,
                          void* ws, long long ws_bytes, double* out, void* stream);
 
+/* The same with a percentile of the pooled surface distances (medpy.metric.binary.hd95 at q = 95).  For each class, with dA, dB
+ * and d(., .) as above, D is the multiset {d(v, dB) : v in dA} + {d(v, dA) : v in dB} of n = |dA| + |dB| values and
+ *   out[(c-1)*7 + 0..5] = the six values pnp_surface_distance writes, bit-identical to it (the same kernels compute them);
+ *   out[(c-1)*7 + 6]    = HD_q = numpy.percentile(D, q) with numpy's default `linear` method, operation for operation:
+ *     qf = q / 100 and v = (n - 1) * qf, each rounded in fp64; lo = floor(v), hi = lo + 1, both n - 1 when v >= n - 1;
+ *     gamma = v - lo, a = D(lo), b = D(hi) (order statistics, 0-based), delta = b - a;
+ *     HD_q = b - delta * (1 - gamma) if gamma >= 0.5, else a + delta * gamma, each difference, product and sum rounded alone.
+ * HD_q is NaN when dA or dB is empty.  q = 100 gives HD, q = 0 the smallest distance.  This is the pooled form (medpy's); the
+ * larger of the two directed percentiles (MONAI) and the surfel-area-weighted form are other metrics.  The order statistics are
+ * found on the device by a radix select over the distances' bit patterns with integer counts only, so HD_q is an exact function
+ * of D and repeated calls are bit-identical; the call only enqueues work (no synchronisation, no copy to the host).
+ *
+ * q must be finite and in [0, 100], else PNP_ERR_BAD_ARG; every other check is pnp_surface_distance's, against this workspace:
+ *   bytes = pnp_surface_distance_workspace's + A(16N) + A(8L) + A(8 ceil(2L / 256)) + A(16584)
+ *   (~30 bytes per voxel: 506 MB at 256^3, for any C).  On any error nothing is launched and out is untouched. */
+int pnp_surface_distance_pct_workspace(int n0, int n1, int n2, int C, long long* bytes /* host */);
+int pnp_surface_distance_pct(const uint8_t* pred, const uint8_t* gt, int n0, int n1, int n2, int C, const double* spacing /* host, 3 */,
+                             double q, void* ws, long long ws_bytes, double* out, void* stream);
+
 /* ---- data preparation: planes resampled out of a volume (resample.cu) ----------------------------------------------------------
  * The augmented coronal slices of the data preparation (preprocess.py; the reference only describes it, README step 1) in one launch
  * per batch.  vol is fp32 and cls uint8 class ids, both C-order [n0][n1][n2] (n2 fastest) on the device.  Output plane p = b*C + k

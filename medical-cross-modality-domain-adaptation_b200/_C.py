@@ -103,6 +103,8 @@ SIGNATURES = {
     "pnp_fill": [P, c_float, c_ll, P],
     "pnp_surface_distance_workspace": [c_int, c_int, c_int, c_int, P],
     "pnp_surface_distance": [P, P, c_int, c_int, c_int, c_int, P, P, c_ll, P, P],
+    "pnp_surface_distance_pct_workspace": [c_int, c_int, c_int, c_int, P],
+    "pnp_surface_distance_pct": [P, P, c_int, c_int, c_int, c_int, P, ctypes.c_double, P, c_ll, P, P],
     "pnp_resample_planes": [P, P, c_int, c_int, c_int, P, c_int, c_int, c_int, c_int, P, P, c_int, P],
     "pnp_native_labels": [P, c_int, c_int, c_int, c_int, P, c_int, c_int, c_int, P, P, P, P],
 }

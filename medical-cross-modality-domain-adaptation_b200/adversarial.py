@@ -541,18 +541,20 @@ class Trainer(object):
                                                          self.num_cls or self.net.n_class, flip_correction, True, rng)
         return dice, jac, cm.astype(np.int64), pred_vol
 
-    def test_eval(self, output_path, flip_correction=True, save_result=False, surface_metrics=False):
+    def test_eval(self, output_path, flip_correction=True, save_result=False, surface_metrics=False, hd_percentile=None):
         """adversarial.py:993-1052: every (label, image) .nii pair of `test_label_list` / `test_nii_list` through the per-subject
         protocol above; writes the summed confusion matrix to <output_path>/cm.csv and returns sample_metric_stddev's pair.
         `save_result` (the segmenter trainer's switch, source_segmenter.py:625-626) also writes the predictions as .nii.gz.
         `surface_metrics` also scores every subject's prediction by per-organ ASSD / HD on the GPU (evaluation.surface_distances,
         voxel units), keeps them in `self.sample_surface_list`, prints their mean and spread and writes
-        <output_path>/surface.csv; the return value and the Dice / Jaccard output are unchanged."""
+        <output_path>/surface.csv; the return value and the Dice / Jaccard output are unchanged.  `hd_percentile` q (95: HD95; only with `surface_metrics`, else ValueError) also
+        scores the q-th percentile of the pooled surface distances: an `hd_pct` entry per subject, `hd<q>` lines and columns."""
         from . import evaluation
         nc = self.num_cls or self.net.n_class
         res = evaluation.run_test_eval(
             self._predict_ct, self.test_label_list, self.test_nii_list, self.net.batch_size, nc,
-            output_path, "dense_pred", flip_correction, save_result, shuffle=True, write_cm=True, surface_metrics=surface_metrics)
+            output_path, "dense_pred", flip_correction, save_result, shuffle=True, write_cm=True, surface_metrics=surface_metrics,
+            hd_percentile=hd_percentile)
         self.sample_eval_list = res[0]
         out = self.sample_metric_stddev(res[0])
         if surface_metrics:
@@ -561,23 +563,24 @@ class Trainer(object):
             evaluation.write_surface_csv(os.path.join(output_path, "surface.csv"), res[2], nc)
         return out
 
-    def test_native(self, pairs, output_path):
+    def test_native(self, pairs, output_path, hd_percentile=None):
         """every raw (image, label) pair segmented on its own grid by the adapted CT stream (native.run): writes
         <output_path>/native_pred/<name>_label.nii.gz and native.csv, prints per-organ Dice and ASSD / HD in mm -> per-subject
-        results"""
+        results.  `hd_percentile` q also scores the q-th percentile HD in mm (native.csv column <organ>_hd<q>_mm)."""
         from . import native
-        return native.run(self._ct_logits, pairs, output_path, self.net.batch_size, self.num_cls or self.net.n_class)
+        return native.run(self._ct_logits, pairs, output_path, self.net.batch_size, self.num_cls or self.net.n_class,
+                          hd_percentile)
 
     def sample_metric_stddev(self, sample_eval_list):
         """adversarial.py:1054-1084"""
         from . import evaluation
         return evaluation.sample_metric_stddev(sample_eval_list, self.num_cls or self.net.n_class)
 
-    def test_model(self, this_model, output_path, surface_metrics=False):
+    def test_model(self, this_model, output_path, surface_metrics=False, hd_percentile=None):
         """adversarial.py:1097-1108: restore a checkpoint, run the test protocol"""
         self.net.restore(this_model)
         logging.info("model has been loaded!")
-        dice, jac = self.test_eval(output_path, surface_metrics=surface_metrics)
+        dice, jac = self.test_eval(output_path, surface_metrics=surface_metrics, hd_percentile=hd_percentile)
         logging.info("testing finished")
         return dice, jac
 

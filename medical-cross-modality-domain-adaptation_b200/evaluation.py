@@ -96,18 +96,24 @@ def eval_volume(predict, raw, raw_y, batch_size, num_cls, flip_correction=True, 
 SURFACE_COLUMNS = ("assd", "hd", "asd_pred_gt", "asd_gt_pred", "border_pred", "border_gt")
 
 
-def surface_distances(pred_vol, gt_vol, num_cls, spacing=None):
+def surface_distances(pred_vol, gt_vol, num_cls, spacing=None, hd_percentile=None):
     """Per-organ surface distances of one subject on the GPU (functional.surface_distances): a dict of [num_cls] arrays `assd`,
     `hd`, `asd_pred_gt`, `asd_gt_pred` (background and organs absent from either volume: NaN) and the border voxel counts
     `border_pred`, `border_gt`.  Distances are in voxel units unless `spacing` (three voxel sizes) is given, like SIFA's
-    evaluation.
+    evaluation.  `hd_percentile` q adds `hd_pct`, the q-th percentile of the pooled surface distances (medpy's hd95 at q = 95),
+    and `hd_percentile`.
 
     `pred_vol` as `eval_volume` / `Trainer.test_eval_volume` return it is in the evaluated orientation: flipped along both
     in-plane axes when flip_correction is on.  Flip the ground truth the same way before calling, e.g.
     `surface_distances(pred_vol, np.flip(np.flip(raw_y, 0), 1), num_cls)`.  Frames the protocol never predicts (the first and
     last, and any a short batch drops) are background in `pred_vol` and are scored as such."""
     from .functional import surface_distances as _sd
-    return _sd(pred_vol, gt_vol, num_cls, spacing)
+    return _sd(pred_vol, gt_vol, num_cls, spacing, hd_percentile)
+
+
+def pct_name(q):
+    """column name of the q-th percentile Hausdorff distance: hd95, hd99.5, ..."""
+    return "hd%g" % q
 
 
 def _organ_names(num_cls):
@@ -115,53 +121,74 @@ def _organ_names(num_cls):
     return [names.get(c, "class_%d" % c) for c in range(num_cls)]
 
 
+def _hd_percentile(sample_surface_list):
+    """the percentile the subjects' dicts carry (None: none); every subject must carry the same"""
+    qs = {s.get("hd_percentile") for s in sample_surface_list}
+    if len(qs) > 1:
+        raise ValueError("subjects scored at different HD percentiles: %s" % sorted(qs, key=str))
+    return qs.pop() if qs else None
+
+
 def surface_metric_stddev(sample_surface_list, num_cls, units="voxel units"):
-    """Per-organ spread and mean of ASSD and HD over subjects, printed in the form of sample_metric_stddev's lines.  Subjects where
-    the organ is absent from the prediction or the ground truth (NaN) are left out and counted.  Returns (mean ASSD [num_cls],
-    mean HD [num_cls]), NaN where no subject has the organ in both volumes.  `units` names the distances' unit in the headings."""
+    """Per-organ spread and mean of ASSD and HD over subjects, printed in the form of sample_metric_stddev's lines, and of the
+    percentile HD (`hd95_stddev` / `hd95_mean` lines) when the subjects were scored with one.  Subjects where the organ is absent
+    from the prediction or the ground truth (NaN) are left out and counted.  Returns (mean ASSD [num_cls], mean HD [num_cls]),
+    NaN where no subject has the organ in both volumes.  `units` names the distances' unit in the headings."""
     names = _organ_names(num_cls)
+    q = _hd_percentile(sample_surface_list)
+    label = {"assd": "assd", "hd": "hd"}
+    if q is not None:
+        label["hd_pct"] = pct_name(q)
+    keys = tuple(label)
     stats = {}
-    for key in ("assd", "hd"):
+    for key in keys:
         mat = np.array([s[key] for s in sample_surface_list], np.float64).reshape(len(sample_surface_list), num_cls)
         stats[key] = [mat[~np.isnan(mat[:, c]), c] for c in range(num_cls)]
     print("------- surface distances over subjects (%s) ---- " % units)
     for c in range(1, num_cls):
         print("organ: %s" % names[c])
-        print("assd_stddev: %s" % (np.std(stats["assd"][c]) if len(stats["assd"][c]) else np.nan))
-        print("hd_stddev: %s" % (np.std(stats["hd"][c]) if len(stats["hd"][c]) else np.nan))
+        for key in keys:
+            print("%s_stddev: %s" % (label[key], np.std(stats[key][c]) if len(stats[key][c]) else np.nan))
     print("------- surface distances over subjects (%s) ----  " % units)
-    mean = {k: np.full(num_cls, np.nan) for k in ("assd", "hd")}
+    mean = {k: np.full(num_cls, np.nan) for k in keys}
     for c in range(1, num_cls):
         print("organ: %s" % names[c])
-        for key in ("assd", "hd"):
+        for key in keys:
             if len(stats[key][c]):
                 mean[key][c] = np.mean(stats[key][c])
-        print("assd_mean: %s" % mean["assd"][c])
-        print("hd_mean: %s" % mean["hd"][c])
+            print("%s_mean: %s" % (label[key], mean[key][c]))
         print("skipped subjects (organ absent from prediction or ground truth): %d" % (len(sample_surface_list) - len(stats["assd"][c])))
     print("-------")
     return mean["assd"], mean["hd"]
 
 
 def write_surface_csv(path, sample_surface_list, num_cls):
-    """one row per subject: subject, then <organ>_<column> for every organ and SURFACE_COLUMNS entry (NaN: organ absent)"""
+    """one row per subject: subject, then <organ>_<column> for every organ and SURFACE_COLUMNS entry (NaN: organ absent), and
+    <organ>_hd<q> (hd95 at q = 95) when the subjects were scored with a percentile"""
     names = _organ_names(num_cls)
+    q = _hd_percentile(sample_surface_list)
+    cols = SURFACE_COLUMNS if q is None else SURFACE_COLUMNS + (pct_name(q),)
+    key = {k: k for k in SURFACE_COLUMNS}
+    if q is not None:
+        key[pct_name(q)] = "hd_pct"
     with open(path, "w") as f:
-        f.write(",".join(["subject"] + ["%s_%s" % (names[c], k) for c in range(1, num_cls) for k in SURFACE_COLUMNS]) + "\n")
+        f.write(",".join(["subject"] + ["%s_%s" % (names[c], k) for c in range(1, num_cls) for k in cols]) + "\n")
         for s in sample_surface_list:
             row = [str(s["subject"])]
             for c in range(1, num_cls):
-                row += [str(int(s[k][c])) if k.startswith("border") else repr(float(s[k][c])) for k in SURFACE_COLUMNS]
+                row += [str(int(s[k][c])) if k.startswith("border") else repr(float(s[key[k]][c])) for k in cols]
             f.write(",".join(row) + "\n")
     return path
 
 
 def run_test_eval(predict, test_label_list, test_nii_list, batch_size, num_cls, output_path, pred_subdir, flip_correction=True,
-                  save_result=False, shuffle=True, write_cm=False, rng=None, surface_metrics=False):
+                  save_result=False, shuffle=True, write_cm=False, rng=None, surface_metrics=False, hd_percentile=None):
     """The subject loop of both `test_eval`s.  Returns (sample_eval_list, summed confusion matrix), and with `surface_metrics`
     a third value: per subject the dict of `surface_distances` plus its "subject" (the image file's name), computed on the
     volumes `save_result` writes -- `pred_vol` against the ground truth in the same orientation, labels above the class range
-    as background."""
+    as background.  `hd_percentile` q (with `surface_metrics` only) adds the q-th percentile HD to every subject's dict."""
+    if hd_percentile is not None and not surface_metrics:
+        raise ValueError("hd_percentile is a surface metric: it needs surface_metrics=True")
     pred_folder = os.path.join(output_path, pred_subdir)
     try:
         os.makedirs(pred_folder)
@@ -186,7 +213,7 @@ def run_test_eval(predict, test_label_list, test_nii_list, batch_size, num_cls, 
             _save_nii_prediction(gth.astype(np.int16), pred_vol.astype(np.int16), nii_fid, pred_folder,
                                  out_bname="dense_pred_" + os.path.basename(str(nii_fid)), num_cls=num_cls)
         if surface_metrics:
-            sd = surface_distances(pred_vol.astype(np.int16), gth.astype(np.int16), num_cls)
+            sd = surface_distances(pred_vol.astype(np.int16), gth.astype(np.int16), num_cls, hd_percentile=hd_percentile)
             sd["subject"] = os.path.basename(str(nii_fid))
             sample_surface_list.append(sd)
     if write_cm:

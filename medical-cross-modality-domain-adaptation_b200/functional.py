@@ -1032,9 +1032,9 @@ def _surface_args(pred, gt, num_cls, spacing):
     return as_u8(pred), as_u8(gt), sp
 
 
-def surface_distances(pred, gt, num_cls, spacing=None):
-    """Per-class surface distances of a predicted label volume against a ground truth (medpy.metric.binary.assd / hd, which
-    the papers' evaluation calls without spacing), on the device.
+def surface_distances(pred, gt, num_cls, spacing=None, hd_percentile=None):
+    """Per-class surface distances of a predicted label volume against a ground truth (medpy.metric.binary.assd / hd / hd95,
+    which the papers' evaluation calls without spacing), on the device.
 
     `pred`, `gt`: host integer arrays [n0, n1, n2] (each n <= 1024); labels outside [0, num_cls) count as background.
     `spacing`: voxel size along the three axes, default 1 (voxel units).  For each class c >= 1 with A = (pred == c) and
@@ -1045,34 +1045,53 @@ def surface_distances(pred, gt, num_cls, spacing=None):
       hd           the larger of the two maxima;
       border_pred / border_gt  |dA| / |dB| (int64).
     Index 0 (background) and classes absent from pred or gt are NaN; the border counts say which side was empty.
-    One upload of each volume, one pnp_surface_distance call, one copy back."""
+    `hd_percentile` q in [0, 100] also gives `hd_pct`, numpy.percentile(q) of the pooled distances {d(v, dB) : v in dA} and
+    {d(v, dA) : v in dB} (medpy's hd95 at q = 95; q = 100 is `hd`), and `hd_percentile` = q.
+    One upload of each volume, one pnp_surface_distance (or pnp_surface_distance_pct) call, one copy back."""
     p, g, sp = _surface_args(pred, gt, num_cls, spacing)
+    pct = hd_percentile is not None
+    if pct:
+        q = float(hd_percentile)
+        if not (math.isfinite(q) and 0.0 <= q <= 100.0):
+            raise ValueError("surface_distances: hd_percentile must be a number in [0, 100], got %r" % (hd_percentile,))
     n0, n1, n2 = p.shape
     nbytes = ctypes.c_longlong(0)
-    call("pnp_surface_distance_workspace", n0, n1, n2, num_cls, ctypes.byref(nbytes))
+    call("pnp_surface_distance_pct_workspace" if pct else "pnp_surface_distance_workspace", n0, n1, n2, num_cls, ctypes.byref(nbytes))
     dev = rt.device()
     dp, dg = torch.from_numpy(p).to(dev), torch.from_numpy(g).to(dev)
     ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
-    out = torch.empty((num_cls - 1) * 6, dtype=torch.float64, device=dev)
-    call("pnp_surface_distance", ptr(dp), ptr(dg), n0, n1, n2, num_cls, (ctypes.c_double * 3)(*sp), ptr(ws), nbytes.value,
-         ptr(out), rt.stream())
-    return surface_from_raw(out.cpu().numpy().reshape(num_cls - 1, 6))
+    cols = 7 if pct else 6
+    out = torch.empty((num_cls - 1) * cols, dtype=torch.float64, device=dev)
+    sp = (ctypes.c_double * 3)(*sp)
+    if pct:
+        call("pnp_surface_distance_pct", ptr(dp), ptr(dg), n0, n1, n2, num_cls, sp, q, ptr(ws), nbytes.value, ptr(out), rt.stream())
+    else:
+        call("pnp_surface_distance", ptr(dp), ptr(dg), n0, n1, n2, num_cls, sp, ptr(ws), nbytes.value, ptr(out), rt.stream())
+    res = surface_from_raw(out.cpu().numpy().reshape(num_cls - 1, cols))
+    if pct:
+        res["hd_percentile"] = q
+    return res
 
 
 def surface_from_raw(raw):
-    """surface_distances' per-class dict from pnp_surface_distance's out[C-1][6] table"""
+    """surface_distances' per-class dict from pnp_surface_distance's out[C-1][6] table, or from pnp_surface_distance_pct's
+    out[C-1][7] (which adds `hd_pct`)"""
     raw = np.asarray(raw, np.float64)
     C = raw.shape[0] + 1
     res = {k: np.full(C, np.nan) for k in SURFACE_KEYS}
     res["border_pred"] = np.zeros(C, np.int64)
     res["border_gt"] = np.zeros(C, np.int64)
+    if raw.shape[1] == 7:
+        res["hd_pct"] = np.full(C, np.nan)
     for c in range(1, C):
-        s_pg, n_p, max_pg, s_gp, n_g, max_gp = raw[c - 1]
+        s_pg, n_p, max_pg, s_gp, n_g, max_gp = raw[c - 1, :6]
         res["border_pred"][c], res["border_gt"][c] = int(n_p), int(n_g)
         if n_p > 0 and n_g > 0:
             res["asd_pred_gt"][c], res["asd_gt_pred"][c] = s_pg / n_p, s_gp / n_g
             res["assd"][c] = (res["asd_pred_gt"][c] + res["asd_gt_pred"][c]) / 2.0
             res["hd"][c] = max(max_pg, max_gp)
+            if raw.shape[1] == 7:
+                res["hd_pct"][c] = raw[c - 1, 6]
     return res
 
 

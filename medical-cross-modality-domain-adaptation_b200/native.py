@@ -12,9 +12,10 @@ for the prepared test split), and a label map of that same scan comes out:
   prepared coordinate map is the inverse of Subject.base composed with to_coronal's permutation and flip, computed in fp64 from
   the subject's own geometry and rounded to fp32 once.
 * scoring against preprocess.map_labels of the native label volume: per-class Dice / Jaccard from the kernel's confusion counts,
-  ASSD / HD in mm from functional.surface_distances with the native voxel sizes (the column norms of the image's affine).
+  ASSD / HD in mm from functional.surface_distances with the native voxel sizes (the column norms of the image's affine), and
+  on request the q-th percentile HD in mm (HD95 at q = 95).
 * outputs under <out>/: native_pred/<name>_label.nii.gz (int16 MMWHS codes 205 / 420 / 500 / 820 for classes 1-4, 0 elsewhere,
-  with the image's shape and affine) and native.csv (one row per subject).
+  with the image's shape and affine) and native.csv (one row per subject; <organ>_hd<q>_mm columns when a percentile is asked).
 
 The crop is the ground-truth heart box, as for the prepared test split: a native-grid score is that of a prediction made inside a
 ground-truth region of interest."""
@@ -109,9 +110,9 @@ def native_prediction(subject, scores, gt):
     return labels, cm.cpu().numpy()
 
 
-def surface_mm(subject, labels, gt, num_cls):
+def surface_mm(subject, labels, gt, num_cls, hd_percentile=None):
     """functional.surface_distances of the native prediction against the native ground truth, in mm"""
-    return F.surface_distances(labels, gt, num_cls, spacing=native_spacing(subject))
+    return F.surface_distances(labels, gt, num_cls, spacing=native_spacing(subject), hd_percentile=hd_percentile)
 
 
 def write_prediction(subject, labels, out_dir, num_cls):
@@ -121,7 +122,7 @@ def write_prediction(subject, labels, out_dir, num_cls):
     return path
 
 
-def evaluate_subject(logits_fn, image_path, label_path, out_dir, batch_size, num_cls):
+def evaluate_subject(logits_fn, image_path, label_path, out_dir, batch_size, num_cls, hd_percentile=None):
     """one subject end to end -> dict: subject, dice, jaccard, cm, the surface_distances fields, the prediction's path"""
     s = preprocess.Subject(image_path, label_path)
     scores = predict_scores(s, logits_fn, batch_size, num_cls)
@@ -129,32 +130,38 @@ def evaluate_subject(logits_fn, image_path, label_path, out_dir, batch_size, num
     labels, cm = native_prediction(s, scores, gt)
     del scores
     labels, gt = labels.cpu().numpy(), gt.cpu().numpy()
-    res = surface_mm(s, labels, gt, num_cls)
+    res = surface_mm(s, labels, gt, num_cls, hd_percentile)
     res.update(subject=s.name, dice=_dice(cm), jaccard=_jaccard(cm), cm=cm, path=write_prediction(s, labels, out_dir, num_cls))
     logging.info("%s: native grid %s, %d prepared frames, Dice %s", s.name, s.native_shape, s.D, np.round(res["dice"], 4))
     return res
 
 
 def write_csv(path, results, num_cls):
-    """one row per subject: subject, then <organ>_<column> for every organ and CSV_COLUMNS entry (NaN: organ absent)"""
+    """one row per subject: subject, then <organ>_<column> for every organ and CSV_COLUMNS entry (NaN: organ absent), and
+    <organ>_hd<q>_mm when the subjects were scored with a percentile"""
     names = evaluation._organ_names(num_cls)
+    q = evaluation._hd_percentile(results)
+    cols = CSV_COLUMNS if q is None else CSV_COLUMNS + (evaluation.pct_name(q) + "_mm",)
     with open(path, "w") as f:
-        f.write(",".join(["subject"] + ["%s_%s" % (names[c], k) for c in range(1, num_cls) for k in CSV_COLUMNS]) + "\n")
+        f.write(",".join(["subject"] + ["%s_%s" % (names[c], k) for c in range(1, num_cls) for k in cols]) + "\n")
         for r in results:
             row = [str(r["subject"])]
             for c in range(1, num_cls):
                 row += [repr(float(r["dice"][c])), repr(float(r["assd"][c])), repr(float(r["hd"][c])), str(int(r["border_pred"][c])),
                         str(int(r["border_gt"][c]))]
+                if q is not None:
+                    row.append(repr(float(r["hd_pct"][c])))
             f.write(",".join(row) + "\n")
     return path
 
 
-def run(logits_fn, pairs, output_path, batch_size, num_cls):
+def run(logits_fn, pairs, output_path, batch_size, num_cls, hd_percentile=None):
     """every (image, label) pair through evaluate_subject; writes <output_path>/native_pred/*.nii.gz and native.csv, prints the
-    per-organ mean and spread of Dice / Jaccard and of ASSD / HD in mm -> the per-subject results"""
+    per-organ mean and spread of Dice / Jaccard and of ASSD / HD (and the `hd_percentile`-th percentile HD) in mm -> the
+    per-subject results"""
     pred_dir = os.path.join(output_path, "native_pred")
     os.makedirs(pred_dir, exist_ok=True)
-    results = [evaluate_subject(logits_fn, im, lb, pred_dir, batch_size, num_cls) for im, lb in pairs]
+    results = [evaluate_subject(logits_fn, im, lb, pred_dir, batch_size, num_cls, hd_percentile) for im, lb in pairs]
     write_csv(os.path.join(output_path, "native.csv"), results, num_cls)
     evaluation.sample_metric_stddev([(r["dice"], r["jaccard"]) for r in results], num_cls)
     evaluation.surface_metric_stddev(results, num_cls, units="mm")
@@ -192,10 +199,12 @@ def main(argv=None):
     ap.add_argument("--pairs", required=True, help="text file of `image_path label_path` lines (as prepare_data.py reads)")
     ap.add_argument("--out", required=True)
     ap.add_argument("--batch-size", type=int, default=8, help="frames per forward call")
+    ap.add_argument("--hd-percentile", type=float, default=None, metavar="Q",
+                    help="also score the Q-th percentile Hausdorff distance in mm (95: HD95; native.csv column <organ>_hd<Q>_mm)")
     a = ap.parse_args(argv)
     logging.basicConfig(level=logging.INFO)
     trainer = build_trainer(a.trainer, a.checkpoint, a.batch_size)
     os.makedirs(a.out, exist_ok=True)
-    results = trainer.test_native(preprocess.read_pairs(a.pairs), a.out)
+    results = trainer.test_native(preprocess.read_pairs(a.pairs), a.out, a.hd_percentile)
     print(os.path.join(a.out, "native.csv"))
     return results

@@ -417,16 +417,18 @@ class Trainer(object):
                                                          flip_correction, False)
         return dice, jac, cm.astype(np.int64), pred_vol
 
-    def test_eval(self, output_path, flip_correction=True, save_result=False, surface_metrics=False):
+    def test_eval(self, output_path, flip_correction=True, save_result=False, surface_metrics=False, hd_percentile=None):
         """source_segmenter.py:572-632: inference on the (label, image) .nii pairs of test_label_list / test_nii_list; with
         `save_result` the dense predictions and ground truths go to <output_path>/test_pred as .nii.gz.  `surface_metrics` also
         scores every subject by per-organ ASSD / HD on the GPU (evaluation.surface_distances, voxel units), keeps them in
         `self.sample_surface_list`, prints their mean and spread and writes <output_path>/surface.csv; the return value and
-        the Dice / Jaccard output are unchanged."""
+        the Dice / Jaccard output are unchanged.  `hd_percentile` q (95: HD95; only with `surface_metrics`, else ValueError) also
+        scores the q-th percentile of the pooled surface distances: an `hd_pct` entry per subject, `hd<q>` lines and columns."""
         from . import evaluation
         res = evaluation.run_test_eval(self._predict, self.test_label_list, self.test_nii_list, self.net.batch_size,
                                        self.num_cls, output_path, "test_pred", flip_correction, save_result,
-                                       shuffle=False, write_cm=False, surface_metrics=surface_metrics)
+                                       shuffle=False, write_cm=False, surface_metrics=surface_metrics,
+                                       hd_percentile=hd_percentile)
         self.sample_eval_list = res[0]
         out = self.sample_metric_stddev(res[0])
         if surface_metrics:
@@ -435,21 +437,22 @@ class Trainer(object):
             evaluation.write_surface_csv(os.path.join(output_path, "surface.csv"), res[2], self.num_cls)
         return out
 
-    def test_native(self, pairs, output_path):
+    def test_native(self, pairs, output_path, hd_percentile=None):
         """every raw (image, label) pair segmented on its own grid (native.run): writes <output_path>/native_pred/<name>_label.nii.gz
-        and native.csv, prints per-organ Dice and ASSD / HD in mm -> per-subject results"""
+        and native.csv, prints per-organ Dice and ASSD / HD in mm -> per-subject results.  `hd_percentile` q also scores the q-th
+        percentile HD in mm (native.csv column <organ>_hd<q>_mm)."""
         from . import native
-        return native.run(self._logits, pairs, output_path, self.net.batch_size, self.num_cls)
+        return native.run(self._logits, pairs, output_path, self.net.batch_size, self.num_cls, hd_percentile)
 
     def sample_metric_stddev(self, sample_eval_list):
         """source_segmenter.py:634-664"""
         from . import evaluation
         return evaluation.sample_metric_stddev(sample_eval_list, self.num_cls)
 
-    def test_choose_model(self, this_model, output_path, surface_metrics=False):
+    def test_choose_model(self, this_model, output_path, surface_metrics=False, hd_percentile=None):
         """source_segmenter.py:666-675: restore a checkpoint, run the test protocol"""
         self.net.restore(this_model)
         logging.info("model has been loaded!")
-        dice, jac = self.test_eval(output_path, surface_metrics=surface_metrics)
+        dice, jac = self.test_eval(output_path, surface_metrics=surface_metrics, hd_percentile=hd_percentile)
         logging.info("testing finished")
         return dice, jac

@@ -7,11 +7,14 @@ bench_volume_source.py -- is written as .nii.gz to a temporary directory.  The s
 * the subject end to end with the GAN trainer's adapted CT stream at B = 8 (seeded initialisation; the time does not depend on
   the weights), split into loading and cropping the subject, prediction of every prepared frame, loading and uploading the native
   ground truth, resampling onto the native grid (the launch and the copy back), surface distances in mm, and the NIfTI write
-  (host clock around work that ends in a device synchronise).
+  (host clock around work that ends in a device synchronise);
+* with `--hd-percentile Q`, surface distances in mm with the Q-th percentile HD end to end, and pnp_surface_distance_pct next to
+  pnp_surface_distance on the native prediction and ground truth at native spacing (bench_surface_distance.compare_pct: CUDA
+  events, `--rounds` alternating rounds of `--calls` calls).
 
 Prints the card name and its power limit with the numbers, one JSON line at the end.
 
-    python scripts/bench_native_eval.py [--launches 200] [--batch-size 8]
+    python scripts/bench_native_eval.py [--launches 200] [--batch-size 8] [--hd-percentile 95 [--calls 5] [--rounds 3]]
 """
 import argparse
 import json
@@ -31,6 +34,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--launches", type=int, default=200)
     ap.add_argument("--batch-size", type=int, default=8)
+    ap.add_argument("--hd-percentile", type=float, default=None, metavar="Q", help="also time pnp_surface_distance_pct at Q")
+    ap.add_argument("--calls", type=int, default=5, help="calls per round of the --hd-percentile comparison")
+    ap.add_argument("--rounds", type=int, default=3, help="alternating rounds of the --hd-percentile comparison")
     a = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "this benchmark measures the GPU and needs one"
@@ -88,6 +94,12 @@ def main():
     res.update(kernel_ms=k_ms, kernel_launches=a.launches, native_voxels=voxels, kernel_Gvoxel_per_s=voxels / k_ms * 1e-6)
     print("pnp_native_labels: %.3f ms per launch over %d launches, %.1f G native voxels/s (%d voxels, %d classes, with counts)" % (
         k_ms, a.launches, voxels / k_ms * 1e-6, voxels, nc))
+    if a.hd_percentile is not None:
+        from bench_surface_distance import compare_pct, print_pct
+        _, res["surface_distances_pct_s"] = clock(lambda: native.surface_mm(s, labels, gt, nc, a.hd_percentile))
+        print("surface distances with hd%g: %.3f s end to end" % (a.hd_percentile, res["surface_distances_pct_s"]))
+        res["pct"] = compare_pct(out, gt_dev, nc, a.hd_percentile, a.calls, a.rounds, native.native_spacing(s))
+        print_pct(res["pct"])
     shutil.rmtree(tmp, ignore_errors=True)
     print(json.dumps(res))
 

@@ -5,11 +5,14 @@ ground truth and a shifted, resized, speckled copy as the prediction, five class
 * the pnp_surface_distance launch sequence alone: CUDA events around `--calls` back-to-back calls after warm-up, per call;
 * `surface_distances` end to end (upload of both volumes, the call, the copy back; host clock, median of `--calls`);
 * the scipy.ndimage form of oracle/surface_exact.py on the same subject on the host cores (one process per organ), and the
-  largest relative difference between the two results.
+  largest relative difference between the two results;
+* with `--hd-percentile Q`, pnp_surface_distance_pct (the same plus the Q-th percentile HD) next to pnp_surface_distance: both
+  timed by CUDA events in `--rounds` alternating rounds of `--calls` calls each (median per call), and whether the six shared
+  columns came out bit-identical.
 
 Prints the card name and its power limit with the numbers, one JSON line at the end.
 
-    python scripts/bench_surface_distance.py [--calls 20] [--depths 256,131] [--no-scipy]
+    python scripts/bench_surface_distance.py [--calls 20] [--depths 256,131] [--no-scipy] [--hd-percentile 95 [--rounds 5]]
 """
 import argparse
 import json
@@ -60,11 +63,66 @@ def _scipy_class(args):
     return scipy_raw((pred == c).astype(np.uint8), (gt == c).astype(np.uint8), 2)[0]
 
 
+def compare_pct(dp, dg, num_cls, q, calls, rounds, spacing=None):
+    """pnp_surface_distance and pnp_surface_distance_pct on the same device volumes (uint8), alternating: CUDA events around
+    `calls` calls per round, `rounds` rounds each -> dict of per-call medians, the rounds, the percentile values and whether the
+    six shared columns are bit-identical"""
+    import ctypes
+    import torch
+    from pnp_b200 import _C, runtime as rt
+    n0, n1, n2 = dp.shape
+    sp = None if spacing is None else (ctypes.c_double * 3)(*[float(x) for x in spacing])
+    ws, out = {}, {}
+    for k, name, cols in (("base", "pnp_surface_distance_workspace", 6), ("pct", "pnp_surface_distance_pct_workspace", 7)):
+        nb = ctypes.c_longlong(0)
+        _C.call(name, n0, n1, n2, num_cls, ctypes.byref(nb))
+        ws[k] = torch.empty(nb.value, dtype=torch.uint8, device=dp.device)
+        out[k] = torch.empty((num_cls - 1) * cols, dtype=torch.float64, device=dp.device)
+    fns = {
+        "base": lambda: _C.call("pnp_surface_distance", dp.data_ptr(), dg.data_ptr(), n0, n1, n2, num_cls, sp, ws["base"].data_ptr(),
+                                ws["base"].numel(), out["base"].data_ptr(), rt.stream()),
+        "pct": lambda: _C.call("pnp_surface_distance_pct", dp.data_ptr(), dg.data_ptr(), n0, n1, n2, num_cls, sp, float(q),
+                               ws["pct"].data_ptr(), ws["pct"].numel(), out["pct"].data_ptr(), rt.stream()),
+    }
+    for fn in fns.values():
+        for _ in range(3):
+            fn()
+    torch.cuda.synchronize()
+    times = {k: [] for k in fns}
+    for _ in range(rounds):
+        for k, fn in fns.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(calls):
+                fn()
+            e1.record()
+            torch.cuda.synchronize()
+            times[k].append(e0.elapsed_time(e1) / calls)
+    six = out["base"].cpu().numpy().reshape(num_cls - 1, 6)
+    seven = out["pct"].cpu().numpy().reshape(num_cls - 1, 7)
+    base_ms, pct_ms = float(np.median(times["base"])), float(np.median(times["pct"]))
+    return {"hd_percentile": float(q), "calls_per_round": calls, "rounds": rounds,
+            "pct_workspace_mb": round(ws["pct"].numel() / 2 ** 20, 1),
+            "base_kernel_ms_rounds": [round(t, 3) for t in times["base"]], "pct_kernel_ms_rounds": [round(t, 3) for t in times["pct"]],
+            "base_kernel_ms": round(base_ms, 3), "pct_kernel_ms": round(pct_ms, 3), "pct_extra_ms": round(pct_ms - base_ms, 3),
+            "hd_pct": [round(float(x), 4) for x in seven[:, 6]], "pooled_n": [int(x) for x in seven[:, 1] + seven[:, 4]],
+            "six_columns_bit_identical": bool(six.tobytes() == np.ascontiguousarray(seven[:, :6]).tobytes())}
+
+
+def print_pct(r):
+    print("  --hd-percentile %g: pnp_surface_distance %.3f ms, pnp_surface_distance_pct %.3f ms per call (+%.3f ms; medians of "
+          "%d alternating rounds of %d calls), workspace %.1f MiB, hd%g %s, pooled n %s, six columns bit-identical: %s"
+          % (r["hd_percentile"], r["base_kernel_ms"], r["pct_kernel_ms"], r["pct_extra_ms"], r["rounds"], r["calls_per_round"],
+             r["pct_workspace_mb"], r["hd_percentile"], r["hd_pct"], r["pooled_n"], r["six_columns_bit_identical"]))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--depths", default="256,131")
     ap.add_argument("--no-scipy", action="store_true")
+    ap.add_argument("--hd-percentile", type=float, default=None, metavar="Q", help="also time pnp_surface_distance_pct at Q")
+    ap.add_argument("--rounds", type=int, default=5, help="alternating rounds of the --hd-percentile comparison")
     a = ap.parse_args()
     import ctypes
     import torch
@@ -122,6 +180,9 @@ def main():
             row.update(scipy_s=round(scipy_s, 2), scipy_processes=NUM_CLS - 1, max_rel_diff_vs_scipy=rel, border_counts_equal=same_counts)
             print("  scipy.ndimage (%d processes): %.2f s; max relative difference of ASSD / HD vs the GPU: %.3g; border counts "
                   "equal: %s" % (NUM_CLS - 1, scipy_s, rel, same_counts))
+        if a.hd_percentile is not None:
+            row["pct"] = compare_pct(dp, dg, NUM_CLS, a.hd_percentile, a.calls, a.rounds)
+            print_pct(row["pct"])
         results.append(row)
         del dp, dg, ws, out
     print(json.dumps({"card": card, "power_limit": plimit, "subjects": results}))
