@@ -26,8 +26,9 @@ from . import layers as L
 from . import optim
 from . import parallel
 from . import runtime as rt
-from .data import SyntheticSource, to_device
-from .lib import _save
+from . import summary
+from .data import pick_source, to_device
+from .lib import save_checkpoint
 from .networks import FB, FRONT, BACK, SegmenterHalf, SegmenterTail
 
 # feature discriminator stages: (scope, cin, cout, inc_dim, down kernel, down stride)  adversarial.py:337-386
@@ -333,6 +334,7 @@ class Trainer(object):
         self.test_label_list, self.test_nii_list = test_label_list, test_nii_list
         self.dp = parallel.DataParallel()
         self.global_step = 0
+        self._graph = self._d_graph = self._g_graph = None       # captured joint / D / G steps (runtime.StepGraph), None: eager
         self.dis_sub_iter = self.train_config.get("dis_sub_iter", 1)
         self.gen_sub_iter = self.train_config.get("gen_sub_iter", 1)
         # the objectives `dis_loss + dis_reg / dis_sub_iter` are built once from train_config (adversarial.py:644,650); the
@@ -467,7 +469,6 @@ class Trainer(object):
         the reference's tags and appends them to <log_dir>/scalars.jsonl; detail=True also prints per-organ Dice / Jaccard.
         `image_summaries` writes the TRAIN_IMAGE_TAGS panels of this pass's own forwards to the event file after the scalars,
         with the same step (add_summary(summary_str, step); add_summary(summary_img, step))."""
-        import json
         from .lib import _indicator_eval
         net = self.net
         rt.scratch.begin_step()
@@ -493,41 +494,18 @@ class Trainer(object):
         scalars = dict(zip(self.SCALAR_TAGS, vals))
         if detail:
             _indicator_eval(cm.cpu().numpy())
-        if log_dir is not None and self.dp.rank == 0:
-            # summary_writer.add_summary(summary_str, step); add_summary(summary_img, step); flush() (adversarial.py:989-991): a
-            # TensorBoard event file and the same scalars as one JSON line
-            from .summary import FileWriter, image_tags
-            writers = self.__dict__.setdefault("_summary_writers", {})
-            if log_dir not in writers:
-                writers[log_dir] = FileWriter(log_dir)
-            writers[log_dir].add_scalars(scalars, step)
-            if image_summaries:
-                u8 = F.image_summary([(fc_["logits"], "softmax2_argmax", 0), (ct_batch, "channel", 1), (ct_batch_y, "argmax", 0),
-                                      (fm["logits"], "softmax2_argmax", 0), (mr_batch, "channel", 1), (mr_batch_y, "argmax", 0)])
-                writers[log_dir].add_images([(tag, u8[s, i]) for s, name in enumerate(self.TRAIN_IMAGE_TAGS)
-                                             for i, tag in enumerate(image_tags(name, u8.shape[1]))], step)
-            writers[log_dir].flush()
-            with open(os.path.join(log_dir, "scalars.jsonl"), "a") as f:
-                f.write(json.dumps(dict(step=int(step), **scalars)) + "\n")
+        # summary_writer.add_summary(summary_str, step); add_summary(summary_img, step); flush() (adversarial.py:989-991)
+        u8 = None
+        if image_summaries and summary.writes(self, log_dir):
+            u8 = F.image_summary([(fc_["logits"], "softmax2_argmax", 0), (ct_batch, "channel", 1), (ct_batch_y, "argmax", 0),
+                                  (fm["logits"], "softmax2_argmax", 0), (mr_batch, "channel", 1), (mr_batch_y, "argmax", 0)])
+        summary.write_pass(self, log_dir, step, scalars, self.TRAIN_IMAGE_TAGS, u8)
         return scalars
 
     def _ct_logits(self, x):
         """the test protocol's forward: inference-mode adapted CT stream (keep_prob 1, every BN switch off -- the feed of
         adversarial.py:1036-1038), x [B, 256, 256, 3] on the device -> logits [B, 256, 256, C]"""
         return self.net.segment(x, "ct", 1.0, front_bn=False, joint_bn=False)["logits"]
-
-    def _predict_ct(self, vol, sl):
-        """one forward call of the test protocol (_ct_logits) -> (argmax labels, confusion counts [label, prediction]) on the host"""
-        from .lib import _label_decomp
-        nc = self.num_cls or self.net.n_class
-        dev = rt.device()
-        x = torch.from_numpy(np.ascontiguousarray(vol, np.float32)).to(dev)
-        y = _label_decomp(nc, torch.from_numpy(np.ascontiguousarray(sl, np.int64)).to(dev))
-        with torch.no_grad():
-            logits = self._ct_logits(x)
-            cm = F.confusion_counts(logits, y)
-            pred = logits.argmax(3)
-        return pred.cpu().numpy(), cm.cpu().numpy()
 
     def test_eval_volume(self, raw, raw_y, flip_correction=True, shuffle_seed=None):
         """adversarial.py:993-1052 for ONE subject: `raw` [256,256,D] intensity volume, `raw_y` [256,256,D] integer labels (what
@@ -537,8 +515,9 @@ class Trainer(object):
         Returns (per-class Dice, per-class Jaccard, confusion matrix, predicted label volume)."""
         from . import evaluation
         rng = None if shuffle_seed is None else np.random.RandomState(shuffle_seed)
-        dice, jac, cm, pred_vol = evaluation.eval_volume(self._predict_ct, raw, raw_y, self.net.batch_size,
-                                                         self.num_cls or self.net.n_class, flip_correction, True, rng)
+        nc = self.num_cls or self.net.n_class
+        dice, jac, cm, pred_vol = evaluation.eval_volume(evaluation.predictor(self._ct_logits, nc), raw, raw_y, self.net.batch_size,
+                                                         nc, flip_correction, True, rng)
         return dice, jac, cm.astype(np.int64), pred_vol
 
     def test_eval(self, output_path, flip_correction=True, save_result=False, surface_metrics=False, hd_percentile=None):
@@ -550,18 +529,9 @@ class Trainer(object):
         <output_path>/surface.csv; the return value and the Dice / Jaccard output are unchanged.  `hd_percentile` q (95: HD95; only with `surface_metrics`, else ValueError) also
         scores the q-th percentile of the pooled surface distances: an `hd_pct` entry per subject, `hd<q>` lines and columns."""
         from . import evaluation
-        nc = self.num_cls or self.net.n_class
-        res = evaluation.run_test_eval(
-            self._predict_ct, self.test_label_list, self.test_nii_list, self.net.batch_size, nc,
-            output_path, "dense_pred", flip_correction, save_result, shuffle=True, write_cm=True, surface_metrics=surface_metrics,
-            hd_percentile=hd_percentile)
-        self.sample_eval_list = res[0]
-        out = self.sample_metric_stddev(res[0])
-        if surface_metrics:
-            self.sample_surface_list = res[2]
-            evaluation.surface_metric_stddev(res[2], nc)
-            evaluation.write_surface_csv(os.path.join(output_path, "surface.csv"), res[2], nc)
-        return out
+        return evaluation.run_protocol(self, self._ct_logits, self.num_cls or self.net.n_class, output_path, "dense_pred",
+                                       flip_correction, save_result, shuffle=True, write_cm=True, surface_metrics=surface_metrics,
+                                       hd_percentile=hd_percentile)
 
     def test_native(self, pairs, output_path, hd_percentile=None):
         """every raw (image, label) pair segmented on its own grid by the adapted CT stream (native.run): writes
@@ -585,107 +555,51 @@ class Trainer(object):
         return dice, jac
 
     # ---- steps as CUDA graphs -----------------------------------------------------------------------------------------
-    def _capture(self, fn, warmup):
-        """Capture `fn()` (forward, backward, all-reduce, optimizer, clip: ~1 k kernel launches) into one CUDA graph.
-        Dropout seeds, optimizer hyper-state and BN statistics live in device memory, so every replay is a genuinely new
-        training step.  Returns (graph, outputs, the moving statistics the step trains) or (None, None, []) -- loudly -- if
-        capture fails."""
-        try:
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                for _ in range(warmup):
-                    fn()
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            # the per-variable operand caches (bf16 weight planes, transposed SIMT weights) are keyed by a HOST-side version
-            # counter: a hit during capture would record no split kernel and freeze the warm-up buffers into the graph, i.e.
-            # every replay would run on pre-capture weights.  Drop them so the captured step re-derives them from the live
-            # arenas, and keep the variables' versions moving on every replay for eager code that runs later.
-            self._invalidate_operand_caches()
-            # (the moving statistics the captured step trains include the critics', whose gamma / beta the G arena does not hold)
-            before = rt.moving_stat_versions()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                out = fn()
-            return g, out, rt.moving_stats_bumped_since(before)
-        except Exception as e:      # noqa: BLE001 -- any capture problem => eager path, loudly
-            import warnings
-            warnings.warn("CUDA-graph capture of the adversarial step failed (%s: %s); running eagerly" % (type(e).__name__, e))
-            torch.cuda.synchronize()
-            return None, None, []
+    def _capture(self, step, examples, keep_prob, warmup, *arenas):
+        """runtime.capture_step of an adversarial step; a replay bumps `arenas`, and every capture starts with the operand caches
+        of both arenas' variables dropped (the DAM's folded BN coefficients included: its statistics move in the G step)"""
+        return rt.capture_step("adversarial", step, examples, keep_prob, warmup, self.d_vars + self.g_vars, arenas)
 
     def capture_joint_step(self, mr_example, ct_example, keep_prob=0.75, warmup=2):
         """`d_step(mr, ct)` + `g_step(ct_g)` as ONE graph on static input buffers (the warm-up steps are real steps)."""
-        self._gx_mr, self._gx_ct, self._gx_ct_g = mr_example.clone(), ct_example.clone(), ct_example.clone()
-        self._graph, self._graph_out, self._graph_bn = self._capture(
-            lambda: (self.d_step(self._gx_mr, self._gx_ct, keep_prob), self.g_step(self._gx_ct_g, keep_prob)), warmup)
-        self._graph_kp = keep_prob
+        self._graph = self._capture(lambda mr, ct, ct_g: (self.d_step(mr, ct, keep_prob), self.g_step(ct_g, keep_prob)),
+                                    (mr_example, ct_example, ct_example), keep_prob, warmup, self.d_arena, self.g_arena)
         return self._graph is not None
 
     def capture_d_step(self, mr_example, ct_example, keep_prob=0.75, warmup=2):
         """the discriminator update alone (pre-train phase; the n_D inner iterations of train-gan)"""
-        self._dx_mr, self._dx_ct = mr_example.clone(), ct_example.clone()
-        self._d_graph, self._d_graph_out, self._d_graph_bn = self._capture(lambda: self.d_step(self._dx_mr, self._dx_ct, keep_prob), warmup)
-        self._d_graph_kp = keep_prob
+        self._d_graph = self._capture(lambda mr, ct: self.d_step(mr, ct, keep_prob), (mr_example, ct_example), keep_prob, warmup,
+                                      self.d_arena)
         return self._d_graph is not None
 
     def capture_g_step(self, ct_example, keep_prob=0.75, warmup=2):
-        self._gsx_ct = ct_example.clone()
-        self._g_graph, self._g_graph_out, self._g_graph_bn = self._capture(lambda: self.g_step(self._gsx_ct, keep_prob), warmup)
-        self._g_graph_kp = keep_prob
+        self._g_graph = self._capture(lambda ct: self.g_step(ct, keep_prob), (ct_example,), keep_prob, warmup, self.g_arena)
         return self._g_graph is not None
 
     def d_step_replay(self, mr_batch, ct_batch, keep_prob=0.75):
-        if getattr(self, "_d_graph", None) is None or keep_prob != self._d_graph_kp:
+        if not rt.StepGraph.fits(self._d_graph, keep_prob):
             return self.d_step(mr_batch, ct_batch, keep_prob)
-        self._dx_mr.copy_(mr_batch, non_blocking=True)
-        self._dx_ct.copy_(ct_batch, non_blocking=True)
-        self._d_graph.replay()
         self.global_step += 1
-        self._replayed(self._d_graph_bn, self.d_arena)
-        return self._d_graph_out
+        return self._d_graph.replay(mr_batch, ct_batch)
 
     def g_step_replay(self, ct_batch, keep_prob=0.75):
-        if getattr(self, "_g_graph", None) is None or keep_prob != self._g_graph_kp:
+        if not rt.StepGraph.fits(self._g_graph, keep_prob):
             return self.g_step(ct_batch, keep_prob)
-        self._gsx_ct.copy_(ct_batch, non_blocking=True)
-        self._g_graph.replay()
         self.global_step += 1
-        self._replayed(self._g_graph_bn, self.g_arena)
-        return self._g_graph_out
-
-    def _replayed(self, bn_moved, *arenas):
-        """a replay changed these arenas and moving statistics on the device: eager code that follows must not trust its cached
-        operands (weight planes, folded batch-norm coefficients)"""
-        for a in arenas:
-            a.bump_versions()
-        for v in bn_moved:
-            v.pnp_version += 1
+        return self._g_graph.replay(ct_batch)
 
     def release_graphs(self):
-        for n in ("_graph", "_graph_out", "_graph_bn", "_d_graph", "_d_graph_out", "_d_graph_bn", "_g_graph", "_g_graph_out", "_g_graph_bn"):
-            setattr(self, n, None)
-
-    def _invalidate_operand_caches(self):
-        for v in self.d_vars + self.g_vars:
-            v.__dict__.pop("_pnp_planes", None)
-            v.__dict__.pop("_pnp_wT", None)
-            v.__dict__.pop("_pnp_bncoef", None)      # inference-mode BN coefficients of the DAM (its statistics move in the G step)
+        self._graph = self._d_graph = self._g_graph = None
 
     def joint_step(self, mr_batch, ct_batch, keep_prob=0.75, ct_batch_g=None):
         """one full adversarial step (D update + clip, then G update); replays the captured graph when there is one.
         `ct_batch_g`: the fresh CT batch the reference dequeues for the generator update (adversarial.py:869-873);
         None re-uses the D step's CT batch."""
-        if getattr(self, "_graph", None) is not None and keep_prob == self._graph_kp:
-            self._gx_mr.copy_(mr_batch, non_blocking=True)
-            self._gx_ct.copy_(ct_batch, non_blocking=True)
-            self._gx_ct_g.copy_(ct_batch if ct_batch_g is None else ct_batch_g, non_blocking=True)
-            self._graph.replay()
+        ct_g = ct_batch if ct_batch_g is None else ct_batch_g
+        if rt.StepGraph.fits(self._graph, keep_prob):
             self.global_step += 2
-            self._replayed(self._graph_bn, self.d_arena, self.g_arena)
-            return self._graph_out
-        return self.d_step(mr_batch, ct_batch, keep_prob), self.g_step(ct_batch if ct_batch_g is None else ct_batch_g, keep_prob)
+            return self._graph.replay(mr_batch, ct_batch, ct_g)
+        return self.d_step(mr_batch, ct_batch, keep_prob), self.g_step(ct_g, keep_prob)
 
     # ---- checkpoint contents: tf.train.Saver() stores every global variable -- model variables, both optimizers' slots,
     #      learning_rate_node and global_step (adversarial.py:640,662,929) ---------------------------------------------
@@ -713,11 +627,7 @@ class Trainer(object):
         return n
 
     def save(self, save_path, output_path):
-        st = self.checkpoint_state()
-        def write():
-            _save(st, save_path, global_step=self.global_step)
-            _save(st, os.path.join(output_path, "latest"))
-        self.dp.save_checkpoint(write)
+        save_checkpoint(self, save_path, output_path)
 
     @staticmethod
     def loss_value(terms):
@@ -749,19 +659,12 @@ class Trainer(object):
         if self.lr_update_flag:
             self.dis_optimizer.set_lr(self.LR_refresh)
             self.gen_optimizer.set_lr(self.LR_refresh)
-        B = self.batch_size
-        def source(given, files, seed, **kw):
-            if given is not None:
-                return given
-            if files:                  # lists/{mr,ct}_train_list: single-example TFRecord files (README.md:49-64)
-                from .tfrecord import TFRecordSource
-                return TFRecordSource(files, B, seed=seed + self.dp.rank)
-            return SyntheticSource(B, seed=seed + self.dp.rank, num_cls=self.num_cls or 5, **kw)
-        mr_src = source(self.mr_source, self.mr_train_list, 1234)
-        ct_src = source(self.ct_source, self.ct_train_list, 4321, shift=0.3, scale=0.8)
+        B, r, nc = self.batch_size, self.dp.rank, self.num_cls or 5
+        mr_src = pick_source(self.mr_source, self.mr_train_list, B, 1234 + r, nc)
+        ct_src = pick_source(self.ct_source, self.ct_train_list, B, 4321 + r, nc, shift=0.3, scale=0.8)
         # the validation queues of adversarial.py:811-815: the given sources, else lists/{mr,ct}_val_list, else further synthetic streams
-        mr_val = source(self.mr_val_source, self.mr_val_list, 2234)
-        ct_val = source(self.ct_val_source, self.ct_val_list, 5321, shift=0.3, scale=0.8)
+        mr_val = pick_source(self.mr_val_source, self.mr_val_list, B, 2234 + r, nc)
+        ct_val = pick_source(self.ct_val_source, self.ct_val_list, B, 5321 + r, nc, shift=0.3, scale=0.8)
         dev = rt.device()
         dis_interval, gen_interval = cfg.get("dis_interval", 1), cfg.get("gen_interval", 1)
         dis_inc, gen_inc = cfg.get("dis_sub_iter_inc", 0), cfg.get("gen_sub_iter_inc", 0)

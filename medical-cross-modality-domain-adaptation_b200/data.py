@@ -102,5 +102,16 @@ class VolumeSource:
         return x, y
 
 
+def pick_source(given, files, batch_size, seed, num_cls, shift=0.0, scale=1.0):
+    """a trainer's input stream: `given` if there is one, else a TFRecordSource over `files` (the reference's lists/*_list of
+    single-example TFRecord files, README.md:49-64), else a SyntheticSource with this shift / scale / num_cls"""
+    if given is not None:
+        return given
+    if files:
+        from .tfrecord import TFRecordSource
+        return TFRecordSource(files, batch_size, seed=seed)
+    return SyntheticSource(batch_size, seed=seed, shift=shift, scale=scale, num_cls=num_cls)
+
+
 def to_device(x, dev):
     return x.to(dev, non_blocking=True)

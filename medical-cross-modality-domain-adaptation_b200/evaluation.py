@@ -2,7 +2,8 @@
 source_segmenter.py:572-664): NIfTI subjects in, per-organ Dice / Jaccard mean and spread over subjects out.
 
 The network forward is the caller's (`predict(x[B,256,256,3] on the device, one-hot y) -> (argmax labels, confusion counts)`), so the
-adversarial trainer evaluates its adapted CT stream and the segmenter trainer its own graph through the same loop.  Host side only."""
+adversarial trainer evaluates its adapted CT stream and the segmenter trainer its own graph through the same loop (`predictor`
+builds it from a trainer's logits function, `run_protocol` is both trainers' `test_eval`).  The loop itself is host side only."""
 import logging
 import os
 
@@ -221,3 +222,39 @@ def run_test_eval(predict, test_label_list, test_nii_list, batch_size, num_cls, 
     if surface_metrics:
         return sample_eval_list, all_cm, sample_surface_list
     return sample_eval_list, all_cm
+
+
+def predictor(logits_fn, num_cls):
+    """the `predict` of the loops above for a trainer's inference forward `logits_fn` (x [B, 256, 256, 3] on the device -> logits
+    [B, 256, 256, C]): (vol, sl) on the host -> (argmax labels, confusion counts [label, prediction]) on the host"""
+    import torch
+    from . import functional as F, runtime as rt
+    from .lib import _label_decomp
+
+    def predict(vol, sl):
+        dev = rt.device()
+        x = torch.from_numpy(np.ascontiguousarray(vol, np.float32)).to(dev)
+        y = _label_decomp(num_cls, torch.from_numpy(np.ascontiguousarray(sl, np.int64)).to(dev))
+        with torch.no_grad():
+            logits = logits_fn(x)
+            cm = F.confusion_counts(logits, y)
+            pred = logits.argmax(3)
+        return pred.cpu().numpy(), cm.cpu().numpy()
+    return predict
+
+
+def run_protocol(trainer, logits_fn, num_cls, output_path, pred_subdir, flip_correction, save_result, shuffle, write_cm,
+                 surface_metrics, hd_percentile):
+    """Both trainers' `test_eval`: run_test_eval over the trainer's test_label_list / test_nii_list with `logits_fn`, kept in
+    `trainer.sample_eval_list`, then the printed spread; with `surface_metrics` also the surface-distance spread,
+    `trainer.sample_surface_list` and <output_path>/surface.csv.  Returns sample_metric_stddev's pair."""
+    res = run_test_eval(predictor(logits_fn, num_cls), trainer.test_label_list, trainer.test_nii_list, trainer.net.batch_size,
+                        num_cls, output_path, pred_subdir, flip_correction, save_result, shuffle=shuffle, write_cm=write_cm,
+                        surface_metrics=surface_metrics, hd_percentile=hd_percentile)
+    trainer.sample_eval_list = res[0]
+    out = sample_metric_stddev(res[0], num_cls)
+    if surface_metrics:
+        trainer.sample_surface_list = res[2]
+        surface_metric_stddev(res[2], num_cls)
+        write_surface_csv(os.path.join(output_path, "surface.csv"), res[2], num_cls)
+    return out

@@ -221,6 +221,14 @@ def _weight_T(W):
     return wT
 
 
+def drop_operand_caches(variables):
+    """forget the operands cached on these variables (bf16 weight planes, transposed SIMT weights, folded inference-mode batch-norm
+    coefficients), so that their next use re-derives them from the live values"""
+    for v in variables:
+        for attr in ("_pnp_planes", "_pnp_wT", "_pnp_bncoef"):
+            v.__dict__.pop(attr, None)
+
+
 def _conv_flops(g):
     return 2.0 * g.B * g.Ho * g.Wo * g.Cout * g.kh * g.kw * g.Cin
 

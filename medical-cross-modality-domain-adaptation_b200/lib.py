@@ -118,3 +118,14 @@ def _save(state, model_path, global_step=None):
     np.savez(tmp, **state)            # a reader (or a second writer) never sees a half-written checkpoint
     os.replace(tmp, path + ".npz")
     return path + ".npz"
+
+
+def save_checkpoint(trainer, save_path, output_path):
+    """both trainers' save: trainer.checkpoint_state() as <save_path>-<global_step>.npz and <output_path>/latest.npz, written by
+    rank 0 while every rank waits"""
+    st = trainer.checkpoint_state()
+
+    def write():
+        _save(st, save_path, global_step=trainer.global_step)
+        _save(st, os.path.join(output_path, "latest"))
+    trainer.dp.save_checkpoint(write)

@@ -217,16 +217,65 @@ def global_variables():
     return [graph.vars[n] for n in graph.order]
 
 
-def moving_stat_versions():
-    """[(moving statistic, its version)]: taken before a CUDA-graph capture, see moving_stats_bumped_since"""
-    return [(v, v.pnp_version) for v in global_variables() if getattr(v, "pnp_kind", "") == "bn_moving"]
+class StepGraph:
+    """A training step captured as ONE CUDA graph on static input buffers (forward, backward, all-reduce, optimizer, clip: ~1 k
+    kernel launches).  Dropout seeds, optimizer hyper-state and BN statistics live in device memory, so every replay is a
+    genuinely new training step.  A replay runs no host code, so replay() also does the host bookkeeping of the step: it bumps the
+    versions of the variables in `arenas` and of the moving statistics the captured step trained (`moved`), so that eager code
+    that follows re-derives its cached operands (weight planes, folded batch-norm coefficients)."""
+
+    def __init__(self, graph, inputs, out, keep_prob, arenas, moved):
+        self.graph, self.inputs, self.out, self.keep_prob, self.arenas, self.moved = graph, inputs, out, keep_prob, arenas, moved
+
+    @staticmethod
+    def fits(g, keep_prob):
+        """whether `g` (a StepGraph, or None for no graph) replays the step at this keep_prob"""
+        return g is not None and keep_prob == g.keep_prob
+
+    def replay(self, *batches):
+        """copy `batches` into the static inputs, replay -> the captured step's outputs"""
+        for buf, b in zip(self.inputs, batches):
+            buf.copy_(b, non_blocking=True)
+        self.graph.replay()
+        for a in self.arenas:
+            a.bump_versions()
+        for v in self.moved:        # (with a frozen gamma / beta the arena's bump does not reach a batch norm's cache key)
+            v.pnp_version += 1
+        return self.out
 
 
-def moving_stats_bumped_since(snapshot):
-    """the moving statistics whose version moved since `snapshot`, i.e. those of the batch norms that ran in training mode in
-    between.  A captured step bumps them on the host only while it is captured; a replay runs no host code, so whoever replays
-    bumps these (the coefficient cache of a batch norm with frozen gamma / beta keys on nothing else that changes)"""
-    return [v for v, ver in snapshot if v.pnp_version != ver]
+def capture_step(what, step, examples, keep_prob, warmup, variables, arenas, detach=False):
+    """`step(*inputs)` captured as a StepGraph on static copies of `examples`, after `warmup` real steps on a side stream.
+    `variables`: those whose operand caches the step reads; `arenas`: those a replay changes on the device.  `detach` hands the
+    outputs out detached.  Returns None -- loudly -- if the capture fails; the caller then steps eagerly."""
+    from .functional import drop_operand_caches
+    inputs = tuple(x.clone() for x in examples)
+    try:
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(warmup):
+                step(*inputs)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        # the operand caches are keyed by a HOST-side version counter: a hit during capture would record no split kernel and
+        # freeze the warm-up buffers into the graph, i.e. every replay would run on pre-capture weights.  Drop them so the
+        # captured step re-derives them from the live arenas
+        drop_operand_caches(variables)
+        # the moving statistics of the batch norms the step trains move their versions on the host only while it is captured
+        # (they include the critics' in a G step, whose gamma / beta the G arena does not hold)
+        before = [(v, v.pnp_version) for v in global_variables() if v.pnp_kind == "bn_moving"]
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            out = step(*inputs)
+        if detach:
+            out = tuple(t.detach() for t in out)
+        return StepGraph(g, inputs, out, keep_prob, arenas, [v for v, ver in before if v.pnp_version != ver])
+    except Exception as e:      # noqa: BLE001 -- any capture problem => eager path, loudly
+        import warnings
+        warnings.warn("CUDA-graph capture of the %s step failed (%s: %s); running eagerly" % (what, type(e).__name__, e))
+        torch.cuda.synchronize()
+        return None
 
 
 def state_dict():

@@ -20,8 +20,9 @@ from . import layers as L
 from . import runtime as rt
 from . import optim
 from . import parallel
-from .data import SyntheticSource, to_device
-from .lib import _label_decomp, _save
+from . import summary
+from .data import pick_source, to_device
+from .lib import _label_decomp, save_checkpoint
 from .networks import FRONT, BACK, SegmenterHalf, SegmenterTail
 
 raw_size = [256, 256, 3]
@@ -157,6 +158,7 @@ class Trainer(object):
         self.source, self.val_source = source, val_source
         self.global_step = 0
         self.dp = parallel.DataParallel()
+        self._graph = None           # the captured train step (runtime.StepGraph), None: eager
         self._build_optimizer()
 
     def _build_optimizer(self):
@@ -194,48 +196,18 @@ class Trainer(object):
         return wce, dice
 
     def capture_train_step(self, x_example, y_example, keep_prob=0.75, warmup=2):
-        """the Adam step as ONE CUDA graph on static input buffers (the warm-up steps are real steps)"""
-        self._gx, self._gy = x_example.clone(), y_example.clone()
-        self._graph = self._graph_out = None
-        try:
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                for _ in range(warmup):
-                    self.train_step(self._gx, self._gy, keep_prob)
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            for v in self.trainables:          # see adversarial.Trainer._capture: no stale operand caches inside the graph
-                v.__dict__.pop("_pnp_planes", None)
-                v.__dict__.pop("_pnp_wT", None)
-                v.__dict__.pop("_pnp_bncoef", None)
-            before = rt.moving_stat_versions()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                out = self.train_step(self._gx, self._gy, keep_prob)
-            # (the losses are handed out detached, for the reason given in Full_DRN.losses: a later capture must not inherit
-            #  this one's gradient accumulators)
-            self._graph, self._graph_out, self._graph_kp = g, tuple(t.detach() for t in out), keep_prob
-            self._graph_bn = rt.moving_stats_bumped_since(before)
-            return True
-        except Exception as e:      # noqa: BLE001
-            import warnings
-            warnings.warn("CUDA-graph capture of the segmenter step failed (%s: %s); running eagerly" % (type(e).__name__, e))
-            torch.cuda.synchronize()
-            self._graph = None
-            return False
+        """the Adam step as ONE CUDA graph on static input buffers (the warm-up steps are real steps).  The losses are handed out
+        detached, for the reason given in Full_DRN.losses: a later capture must not inherit this one's gradient accumulators."""
+        self._graph = None
+        self._graph = rt.capture_step("segmenter", lambda x, y: self.train_step(x, y, keep_prob), (x_example, y_example),
+                                      keep_prob, warmup, self.trainables, (self.arena,), detach=True)
+        return self._graph is not None
 
     def train_step_replay(self, batch_x, batch_y, keep_prob=0.75):
-        if getattr(self, "_graph", None) is None or keep_prob != self._graph_kp:
+        if not rt.StepGraph.fits(self._graph, keep_prob):
             return self.train_step(batch_x, batch_y, keep_prob)
-        self._gx.copy_(batch_x, non_blocking=True)
-        self._gy.copy_(batch_y, non_blocking=True)
-        self._graph.replay()
         self.global_step += 1
-        self.arena.bump_versions()
-        for v in self._graph_bn:           # (with a frozen gamma / beta the arena's bump does not reach a batch norm's cache key)
-            v.pnp_version += 1
-        return self._graph_out
+        return self._graph.replay(batch_x, batch_y)
 
     # scalar tags of the merged summary op, in its order (source_segmenter.py:387-396)
     SCALAR_TAGS = ("loss", "regularizer_loss", "weighted_loss", "dice_loss", "dice_eval", "dice_eval_c1", "dice_eval_c2", "dice_eval_c3",
@@ -251,32 +223,16 @@ class Trainer(object):
                [float(arr[i]) for i in range(1, 5)]
         return dict(zip(self.SCALAR_TAGS, vals))
 
-    def _write_scalars(self, log_dir, step, scalars, images=None):
+    def _summaries(self, log_dir, step, names, image_summaries, logits, batch_x, batch_y, wce, dice):
         """tf.summary.FileWriter(output_path + '/train_log' | '/val_log').add_summary(scalar_summary_op, step) (source_segmenter.py:
-        464-465, 537-539, 567-569): a TensorBoard event file plus the same numbers as one JSON line; rank 0 only.  `images`
-        (tag, uint8 panel) pairs follow as a second event with the same step, as add_summary(summary_img, step) does"""
-        if log_dir is None or self.dp.rank != 0:
+        464-465, 537-539, 567-569), and with `image_summaries` add_summary(summary_img, step) of the merged image op `names`,
+        rendered from the pass's own tensors -- [compact_pred, x[:,:,:,1], compact_y] (summary.write_pass)"""
+        if log_dir is None:
             return
-        import json
-        from .summary import FileWriter
-        writers = self.__dict__.setdefault("_summary_writers", {})
-        if log_dir not in writers:
-            writers[log_dir] = FileWriter(log_dir)
-        writers[log_dir].add_scalars(scalars, step)
-        if images is not None:
-            writers[log_dir].add_images(images, step)
-        writers[log_dir].flush()
-        with open(os.path.join(log_dir, "scalars.jsonl"), "a") as f:
-            f.write(json.dumps(dict(step=int(step), **scalars)) + "\n")
-
-    def _images(self, log_dir, names, logits, batch_x, batch_y):
-        """the panels of one merged image op from the pass's own tensors -- [compact_pred, x[:,:,:,1], compact_y] -- as
-        (tag, uint8 [H, W]) pairs in the merged op's order; None where nothing is written (no log_dir, or not rank 0)"""
-        if log_dir is None or self.dp.rank != 0:
-            return None
-        from .summary import image_tags
-        u8 = F.image_summary([(logits, "softmax2_argmax", 0), (batch_x, "channel", 1), (batch_y, "argmax", 0)])
-        return [(tag, u8[s, i]) for s, name in enumerate(names) for i, tag in enumerate(image_tags(name, u8.shape[1]))]
+        u8 = None
+        if image_summaries and summary.writes(self, log_dir):
+            u8 = F.image_summary([(logits, "softmax2_argmax", 0), (batch_x, "channel", 1), (batch_y, "argmax", 0)])
+        summary.write_pass(self, log_dir, step, self._scalars(logits, batch_y, wce, dice), names, u8)
 
     def output_minibatch_stats(self, batch_x, batch_y, step=None, log_dir=None, image_summaries=False):
         """source_segmenter.py:525-539: the tensorboard pass on the training batch feeds x, y and keep_prob 1 ONLY -- both BN
@@ -287,9 +243,7 @@ class Trainer(object):
         with torch.no_grad():
             logits = self.net.forward(batch_x, keep_prob=1.0, main_bn=True, adapt_bn=True)
             wce, dice = self.net.losses(logits, batch_y)
-            if log_dir is not None:
-                images = self._images(log_dir, self.TRAIN_IMAGE_TAGS, logits, batch_x, batch_y) if image_summaries else None
-                self._write_scalars(log_dir, step, self._scalars(logits, batch_y, wce, dice), images)
+            self._summaries(log_dir, step, self.TRAIN_IMAGE_TAGS, image_summaries, logits, batch_x, batch_y, wce, dice)
         return self.net.cost_value(wce, dice)
 
     def feed(self, images, raw_labels):
@@ -328,21 +282,9 @@ class Trainer(object):
         else:
             self.dp.broadcast_params(self.optimizer.m)
             self.dp.broadcast_params(self.optimizer.v)
-        if self.source is not None:
-            src = self.source
-        elif self.train_list:      # the reference's lists/*_train_list of single-example TFRecord files
-            from .tfrecord import TFRecordSource
-            src = TFRecordSource(self.train_list, self.batch_size, seed=1234 + self.dp.rank)
-        else:
-            src = SyntheticSource(self.batch_size, seed=1234 + self.dp.rank, num_cls=self.num_cls)
+        src = pick_source(self.source, self.train_list, self.batch_size, 1234 + self.dp.rank, self.num_cls)
         # the validation queue of source_segmenter.py:325,467 (val_list), else a second synthetic stream
-        if self.val_source is not None:
-            val_src = self.val_source
-        elif self.val_list:
-            from .tfrecord import TFRecordSource
-            val_src = TFRecordSource(self.val_list, self.batch_size, seed=4321 + self.dp.rank)
-        else:
-            val_src = SyntheticSource(self.batch_size, seed=4321 + self.dp.rank, num_cls=self.num_cls)
+        val_src = pick_source(self.val_source, self.val_list, self.batch_size, 4321 + self.dp.rank, self.num_cls)
         img = {"image_summaries": True} if image_summaries else {}       # the monitoring calls stay as they were when off
         for epoch in range(epochs):
             for step in range(epoch * training_iters, (epoch + 1) * training_iters):
@@ -371,11 +313,7 @@ class Trainer(object):
         return st
 
     def save(self, save_path, output_path):
-        st = self.checkpoint_state()
-        def write():
-            _save(st, save_path, global_step=self.global_step)
-            _save(st, os.path.join(output_path, "latest"))
-        self.dp.save_checkpoint(write)
+        save_checkpoint(self, save_path, output_path)
 
     def val_stats(self, batch_x, batch_y, step=None, log_dir=None, detail=False, image_summaries=False):
         """source_segmenter.py:541-570: inference-mode forward (BN moving stats, keep_prob 1) on a validation batch; `detail` prints
@@ -388,9 +326,7 @@ class Trainer(object):
             d, arr = self.net.dice_eval(logits, batch_y)
             if detail:
                 _indicator_eval(self.net.confusion_matrix(logits, batch_y).cpu().numpy())
-            if log_dir is not None:
-                images = self._images(log_dir, self.VAL_IMAGE_TAGS, logits, batch_x, batch_y) if image_summaries else None
-                self._write_scalars(log_dir, step, self._scalars(logits, batch_y, wce, dice), images)
+            self._summaries(log_dir, step, self.VAL_IMAGE_TAGS, image_summaries, logits, batch_x, batch_y, wce, dice)
         return {"loss": self.net.cost_value(wce, dice), "dice_eval": float(d), "dice_arr": [float(a) for a in arr]}
 
     # ---- test protocol on NIfTI subjects (source_segmenter.py:572-675) -----------------------------------------------
@@ -399,22 +335,11 @@ class Trainer(object):
         256, 3] on the device -> logits [B, 256, 256, C]"""
         return self.net.forward(x, keep_prob=1.0, main_bn=False, adapt_bn=False)
 
-    def _predict(self, vol, sl):
-        """one forward call of the test protocol (_logits) -> (argmax labels, confusion counts [label, prediction]) on the host"""
-        dev = rt.device()
-        x = torch.from_numpy(np.ascontiguousarray(vol, np.float32)).to(dev)
-        y = _label_decomp(self.num_cls, torch.from_numpy(np.ascontiguousarray(sl, np.int64)).to(dev))
-        with torch.no_grad():
-            logits = self._logits(x)
-            cm = self.net.confusion_matrix(logits, y)
-            pred = logits.argmax(3)
-        return pred.cpu().numpy(), cm.cpu().numpy()
-
     def test_eval_volume(self, raw, raw_y, flip_correction=True):
         """one subject of test_eval: frames in order (see evaluation.subject_batches for the reference's broken loop header)"""
         from . import evaluation
-        dice, jac, cm, pred_vol = evaluation.eval_volume(self._predict, raw, raw_y, self.net.batch_size, self.num_cls,
-                                                         flip_correction, False)
+        dice, jac, cm, pred_vol = evaluation.eval_volume(evaluation.predictor(self._logits, self.num_cls), raw, raw_y,
+                                                         self.net.batch_size, self.num_cls, flip_correction, False)
         return dice, jac, cm.astype(np.int64), pred_vol
 
     def test_eval(self, output_path, flip_correction=True, save_result=False, surface_metrics=False, hd_percentile=None):
@@ -425,17 +350,8 @@ class Trainer(object):
         the Dice / Jaccard output are unchanged.  `hd_percentile` q (95: HD95; only with `surface_metrics`, else ValueError) also
         scores the q-th percentile of the pooled surface distances: an `hd_pct` entry per subject, `hd<q>` lines and columns."""
         from . import evaluation
-        res = evaluation.run_test_eval(self._predict, self.test_label_list, self.test_nii_list, self.net.batch_size,
-                                       self.num_cls, output_path, "test_pred", flip_correction, save_result,
-                                       shuffle=False, write_cm=False, surface_metrics=surface_metrics,
-                                       hd_percentile=hd_percentile)
-        self.sample_eval_list = res[0]
-        out = self.sample_metric_stddev(res[0])
-        if surface_metrics:
-            self.sample_surface_list = res[2]
-            evaluation.surface_metric_stddev(res[2], self.num_cls)
-            evaluation.write_surface_csv(os.path.join(output_path, "surface.csv"), res[2], self.num_cls)
-        return out
+        return evaluation.run_protocol(self, self._logits, self.num_cls, output_path, "test_pred", flip_correction, save_result,
+                                       shuffle=False, write_cm=False, surface_metrics=surface_metrics, hd_percentile=hd_percentile)
 
     def test_native(self, pairs, output_path, hd_percentile=None):
         """every raw (image, label) pair segmented on its own grid (native.run): writes <output_path>/native_pred/<name>_label.nii.gz

@@ -14,6 +14,7 @@ The first record of a file is the version event `brain.Event:2`, as TensorFlow w
 PNGs (`encode_png`, stdlib zlib) of the uint8 panels that functional.image_summary renders on the GPU, tagged as TF-1.4's
 ImageSummaryOp tags them (`image_tags`).  The `graph=sess.graph` GraphDef event is not written.  tests/test_summary_cpu.py and
 tests/test_image_summary_cpu.py read the files back with the `tensorboard` package's own loader."""
+import json
 import os
 import socket
 import struct
@@ -132,3 +133,27 @@ class FileWriter(object):
             self.close()
         except Exception:
             pass
+
+
+def writes(trainer, log_dir):
+    """whether a monitoring pass of `trainer` writes to `log_dir`: only with a log_dir, and only on rank 0"""
+    return log_dir is not None and trainer.dp.rank == 0
+
+
+def write_pass(trainer, log_dir, step, scalars, image_names=(), u8=None):
+    """One monitoring pass of a trainer: add_summary(scalar_summary_op, step), then add_summary(image_summary_op, step), then
+    flush() on the trainer's FileWriter of `log_dir` (one per directory), and the same scalars as one JSON line appended to
+    <log_dir>/scalars.jsonl; nothing unless `writes`.  `u8`: functional.image_summary's panels of the sources named
+    `image_names`, in the merged image op's order, or None for no image event."""
+    if not writes(trainer, log_dir):
+        return
+    writers = trainer.__dict__.setdefault("_summary_writers", {})
+    if log_dir not in writers:
+        writers[log_dir] = FileWriter(log_dir)
+    writers[log_dir].add_scalars(scalars, step)
+    if u8 is not None:
+        writers[log_dir].add_images([(tag, u8[s, i]) for s, name in enumerate(image_names)
+                                     for i, tag in enumerate(image_tags(name, u8.shape[1]))], step)
+    writers[log_dir].flush()
+    with open(os.path.join(log_dir, "scalars.jsonl"), "a") as f:
+        f.write(json.dumps(dict(step=int(step), **scalars)) + "\n")

@@ -340,7 +340,7 @@ def test_segmenter_graph_replay_keeps_the_operands_coherent(frozen_back):
     assert t.capture_train_step(m.x, m.y, 0.75, warmup=2), "CUDA-graph capture failed the second time"
     t.train_step_replay(m.x, m.y, 0.75)
     torch.cuda.synchronize()
-    t._graph = t._graph_out = None
+    t._graph = None
 
 
 @pytest.mark.parametrize("step", ["joint", "d", "g"])
