@@ -1,9 +1,15 @@
 """The model-level builders of the parity tests: the product's segmenter / adversarial network and trainer next to the CPU
-oracle on identical seeded initial variables, and the loss and variable comparisons between them."""
+oracle on identical seeded initial variables, the loss and variable comparisons between them, and the real training steps that
+the in-step taps (tests/test_layer_taps_gpu.py, tests/test_node_taps_gpu.py) run."""
+import json
+import os
+
 import numpy as np
 import torch
 
 from tests.util import l2_err, rel_err
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def bn_noise(P, bns, seed):
@@ -180,3 +186,79 @@ def state_close(rt, oracle, tol, only=None, norm=rel_err, label="worst variable:
     print("  " + label.format(name=wname, err=worst, tol=tol))
     assert worst <= tol, (wname, worst)
     return worst
+
+
+# ------------------------------------------------------------------------------------------------
+# the real training steps of the in-step taps
+# ------------------------------------------------------------------------------------------------
+def reference_trace():
+    with open(os.path.join(GOLDEN, "reference_graph_trace.json")) as f:
+        return json.load(f)
+
+
+def trace_counts(op="conv"):
+    """events of kind `op` ("conv", "maxpool", "fc", "PS") per sub-graph of the reference's recorded graphs"""
+    ref = reference_trace()
+    count = lambda evs: sum(1 for e in evs if e["op"] == op)  # noqa: E731
+    sec = lambda s: [e for e in ref["events"] if e["section"] == s]  # noqa: E731
+    return {"source_segmenter": count(ref["source_segmenter"]["events"]),
+            # one adversarial stream: half of the zip network (the MR and the CT front) + the shared second half
+            "stream": count(sec("create_zip_network#1")) // 2 + count(sec("create_second_half#1")),
+            "classifier": count(sec("create_classifier#1")), "mask_critic": count(sec("create_mask_critic#1"))}
+
+
+def step_images(B, seed, shift=0.0, scale=1.0):
+    from oracle.pnp_graphs import synthetic_images
+    return synthetic_images(B, seed, shift, scale).to("cuda")
+
+
+def step_onehot(B, seed):
+    from oracle.pnp_graphs import synthetic_labels
+    return torch.nn.functional.one_hot(torch.from_numpy(synthetic_labels(B, seed)), 5).float().to("cuda")
+
+
+def build_step(kind, backend, B):
+    """one training step of kind "seg" (segmenter), "d" (pre-train critic step), "g" (generator step), "dg" (critic then
+    generator step) or "eval" (the folded CT evaluation) -> (run(keep_prob), expected (layer_forward, layer_backward, tail forward,
+    tail backward) counts of one run, trainer)"""
+    n = trace_counts()
+    if kind == "seg":
+        net, tr, _, _ = seg_pair(backend, B)
+        x, y = step_images(B, 11), step_onehot(B, 12)
+        ns = n["source_segmenter"]           # the output convolution trains: it runs through layer_forward
+        return (lambda kp: tr.train_step(x, y, kp)), (ns, ns, 0, 0), tr
+    from pnp_b200.train_gan import configure
+    phase = "pre-train" if kind == "d" else "train-gan"
+    lam = configure(phase)[0]["lambda_mask_loss"]
+    net, tr, _ = adv_pair(backend, lam, phase, B, with_oracle=False, critic_keep_prob=0.75)
+    mr, ct, ct2 = step_images(B, 21), step_images(B, 22, 0.3, 0.8), step_images(B, 23, 0.3, 0.8)
+    seg_l = n["stream"] - 1                  # the frozen output convolution runs inside _TailFn
+    critics = n["classifier"] + (n["mask_critic"] if lam else 0)
+    d_counts = (2 * seg_l + 2 * critics, 2 * critics, 2, 0)
+    g_counts = (seg_l + critics, seg_l + critics, 1, 1)
+    if kind == "d":
+        return (lambda kp: tr.d_step(mr, ct, kp)), d_counts, tr
+    if kind == "g":
+        return (lambda kp: tr.g_step(ct2, kp)), g_counts, tr
+    if kind == "dg":
+        return (lambda kp: (tr.d_step(mr, ct, kp), tr.g_step(ct2, kp))), tuple(a + b for a, b in zip(d_counts, g_counts)), tr
+    labels = step_onehot(B, 24)
+    return (lambda kp: tr.evaluate(ct, labels)), (seg_l, 0, 1, 0), tr
+
+
+def prepare_step(monkeypatch, kind, backend, B, keep, seed, mutate=None):
+    """a fresh graph and trainer for build_step's step, the RNG seeded, mutate(monkeypatch, trainer) applied (a negative control),
+    and the step run once untapped, so that the dispatcher has proven its tensor-core geometries -> (run, expected counts,
+    trainer)"""
+    import pnp_b200  # noqa: F401
+    from pnp_b200 import functional as F, runtime as rt
+    rt.reset_default_graph()
+    F._tc_proven.clear()
+    F._tc_declined.clear()
+    run, expect, tr = build_step(kind, backend, B)
+    rt.manual_seed(seed)
+    if mutate is not None:
+        mutate(monkeypatch, tr)
+    run(keep)
+    torch.cuda.synchronize()
+    return run, expect, tr

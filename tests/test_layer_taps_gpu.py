@@ -19,8 +19,6 @@ tests may miss, and each must trip a tap."""
 import collections
 import copy
 import ctypes
-import json
-import os
 import time
 
 import numpy as np
@@ -32,13 +30,13 @@ from oracle import layer_exact as LX
 from oracle import philox
 from oracle import simt_exact as X
 from tests import cabi
+from tests.models import prepare_step
 
 pytestmark = pytest.mark.gpu
 
 DEV = cabi.DEV
 SEED = 4242
 PHILOX_SPOT = 4096           # elements of every site's mask compared with the independent Philox reference
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 # every route of the dispatcher that a step of these graphs takes.  The activation-only backward (an activated convolution without
 # batch norm) is not among them: neither graph has such a layer, so no step calls it.
@@ -51,18 +49,6 @@ def _prod():
     import pnp_b200  # noqa: F401
     from pnp_b200 import functional as F, runtime as rt, _C
     return F, rt, _C
-
-
-def _trace_counts():
-    """convolutions per sub-graph of the reference's recorded graphs"""
-    with open(os.path.join(HERE, "golden", "reference_graph_trace.json")) as f:
-        ref = json.load(f)
-    convs = lambda evs: sum(1 for e in evs if e["op"] == "conv")  # noqa: E731
-    sec = lambda s: [e for e in ref["events"] if e["section"] == s]  # noqa: E731
-    return {"source_segmenter": convs(ref["source_segmenter"]["events"]),
-            # one adversarial stream: half of the zip network (the MR and the CT front) + the shared second half
-            "stream": convs(sec("create_zip_network#1")) // 2 + convs(sec("create_second_half#1")),
-            "classifier": convs(sec("create_classifier#1")), "mask_critic": convs(sec("create_mask_critic#1"))}
 
 
 class Taps:
@@ -431,55 +417,8 @@ def _restore():
 # ------------------------------------------------------------------------------------------------
 # the steps
 # ------------------------------------------------------------------------------------------------
-def _images(B, seed, shift=0.0, scale=1.0):
-    from oracle.pnp_graphs import synthetic_images
-    return synthetic_images(B, seed, shift, scale).to(DEV)
-
-
-def _onehot(B, seed):
-    from oracle.pnp_graphs import synthetic_labels
-    return torch.nn.functional.one_hot(torch.from_numpy(synthetic_labels(B, seed)), 5).float().to(DEV)
-
-
-def _build(kind, backend, B):
-    """-> (run(), expected (layer_forward, layer_backward, tail forward, tail backward) counts of one run)"""
-    from tests.models import adv_pair, seg_pair
-    n = _trace_counts()
-    if kind == "seg":
-        net, tr, _, _ = seg_pair(backend, B)
-        x, y = _images(B, 11), _onehot(B, 12)
-        ns = n["source_segmenter"]           # the output convolution trains: it runs through layer_forward
-        return (lambda kp: tr.train_step(x, y, kp)), (ns, ns, 0, 0)
-    from pnp_b200.train_gan import configure
-    phase = "pre-train" if kind == "d" else "train-gan"
-    lam = configure(phase)[0]["lambda_mask_loss"]
-    net, tr, _ = adv_pair(backend, lam, phase, B, with_oracle=False, critic_keep_prob=0.75)
-    mr, ct, ct2 = _images(B, 21), _images(B, 22, 0.3, 0.8), _images(B, 23, 0.3, 0.8)
-    seg_l = n["stream"] - 1                  # the frozen output convolution runs inside _TailFn
-    critics = n["classifier"] + (n["mask_critic"] if lam else 0)
-    d_counts = (2 * seg_l + 2 * critics, 2 * critics, 2, 0)
-    g_counts = (seg_l + critics, seg_l + critics, 1, 1)
-    if kind == "d":
-        return (lambda kp: tr.d_step(mr, ct, kp)), d_counts
-    if kind == "g":
-        return (lambda kp: tr.g_step(ct2, kp)), g_counts
-    if kind == "dg":
-        return (lambda kp: (tr.d_step(mr, ct, kp), tr.g_step(ct2, kp))), tuple(a + b for a, b in zip(d_counts, g_counts))
-    labels = _onehot(B, 24)
-    return (lambda kp: tr.evaluate(ct, labels)), (seg_l, 0, 1, 0)
-
-
 def _tapped_step(monkeypatch, kind, backend, B, keep, mutate=None):
-    F, rt, _C = _prod()
-    rt.reset_default_graph()
-    F._tc_proven.clear()
-    F._tc_declined.clear()
-    run, expect = _build(kind, backend, B)
-    rt.manual_seed(SEED)
-    if mutate is not None:
-        mutate(monkeypatch)
-    run(keep)                                # untapped: proves the tensor-core geometries
-    torch.cuda.synchronize()
+    run, expect, _ = prepare_step(monkeypatch, kind, backend, B, keep, SEED, mutate)
     taps = Taps(monkeypatch)
     taps.install()
     t0 = time.time()
@@ -554,7 +493,7 @@ def test_steps_reach_every_route():
 # ------------------------------------------------------------------------------------------------
 # negative controls at B = 2
 # ------------------------------------------------------------------------------------------------
-def _stale_scratch(mp):
+def _stale_scratch(mp, tr):
     """(a) begin_step resets the offset but skips the fill: the fp64 BN accumulators carry the previous step's sums"""
     F, rt, _C = _prod()
 
@@ -563,14 +502,14 @@ def _stale_scratch(mp):
     mp.setattr(type(rt.scratch), "begin_step", begin_step)
 
 
-def _drop_plus_one(mp):
+def _drop_plus_one(mp, tr):
     """(b) the backward pass reads its dropout mask from stream id + 1"""
     F, rt, _C = _prod()
     real = F._drop_from
     mp.setattr(F, "_drop_from", lambda info: real(None if info is None else (info[0] + 1, info[1])))
 
 
-def _wrong_act(mp):
+def _wrong_act(mp, tr):
     """(c) the backward pass runs with the activation code of a wrong LayerCfg copy (leaky ReLU <-> ReLU)"""
     F, rt, _C = _prod()
     real = F.layer_backward
@@ -582,7 +521,7 @@ def _wrong_act(mp):
     mp.setattr(F, "layer_backward", bwd)
 
 
-def _no_dx_into(mp):
+def _no_dx_into(mp, tr):
     """(d) _ResBlockFn.backward does not merge the skip gradient into the first convolution's dgrad"""
     F, rt, _C = _prod()
 
