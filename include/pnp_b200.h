@@ -378,6 +378,37 @@ int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0, int n1, in
 int pnp_native_labels(const float* scores, int n0, int n1, int n2, int C, const float* map, int m0, int m1, int m2, uint8_t* out,
                       const uint8_t* gt, long long* cm, void* stream);
 
+/* ---- evaluation: largest connected component per class (components3d.cu) ------------------------------------------------------
+ * The usual clean-up of a segmentation (nnU-Net's post-processing): every structure is one connected body, so only the largest
+ * 3-D connected component of each class is kept and the rest is set to background.  labels, out and gt are uint8 C-order
+ * [n0][n1][n2] (n2 fastest) on the device; labels >= C count as background.  connectivity is 6 (face neighbours) or 26 (face,
+ * edge and corner neighbours): scipy.ndimage.generate_binary_structure(3, 1) and (3, 3).  For each class c in 1 .. C-1:
+ *   the components of c are the connected components of {v : labels[v] == c}; voxels outside the volume belong to nothing;
+ *   the kept component is the one with the most voxels; among equal sizes, the one whose smallest C-order linear index is
+ *   smallest (what np.argmax(np.bincount(ndimage.label(mask, s)[0].ravel())[1:]) selects: scipy numbers components in raster
+ *   order of their first voxel).  A class with no voxels keeps nothing.
+ *   out[v] = c if v lies in the kept component of class c, else 0 (labels >= C become 0).  out may equal labels (in place).
+ *   stats (int64 [C][3], device): stats[c] = (number of components, voxels kept, voxels removed); row 0 is (0, 0, number of labels
+ *     >= C), the voxels set to 0 for being out of range.  The call zeroes stats first.
+ *   cm (int64 [C][C], device, optional with gt): cm[gt][out] counted over every voxel, ground-truth labels >= C as background
+ *     (as pnp_native_labels counts them).  The call zeroes cm first.
+ * Union-find over an int32 parent array: each voxel is linked to its same-class neighbours of smaller linear index (3 for
+ * 6-connectivity, 13 for 26), a root is only hooked under a smaller root (atomicCAS), so every root is the smallest linear index
+ * of its component, and the per-class atomicMax of (size << 32) | (0xFFFFFFFF - root) picks the kept one.  The call only enqueues
+ * a fixed sequence of launches (no synchronisation, no copy to the host); every quantity is an integer, so out, stats and cm are
+ * exact functions of the input and repeated calls are bit-identical.
+ *
+ * NULL labels / out / stats / ws, only one of gt / cm, a non-positive size, or a workspace smaller than
+ * pnp_largest_components_workspace's are PNP_ERR_BAD_ARG; C outside [2, 8], connectivity other than 6 or 26, or n0*n1*n2 >= 2^31
+ * are PNP_ERR_UNSUPPORTED.  On any error nothing is launched and the outputs are untouched.
+ *
+ * Workspace (device, ws_bytes long): with N = n0*n1*n2 and A(x) = x rounded up to a multiple of 256,
+ *   bytes = 2 A(4N) + 256      (parent and size, int32 per voxel, then the per-class keys: ~8 bytes per voxel, 629 MB at
+ *                               512 x 512 x 300, for any C and either connectivity). */
+int pnp_largest_components_workspace(int n0, int n1, int n2, int C, int connectivity, long long* bytes /* host */);
+int pnp_largest_components(const uint8_t* labels, int n0, int n1, int n2, int C, int connectivity, uint8_t* out, const uint8_t* gt,
+                           long long* cm, long long* stats, void* ws, long long ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

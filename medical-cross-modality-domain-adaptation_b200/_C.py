@@ -107,6 +107,8 @@ SIGNATURES = {
     "pnp_surface_distance_pct": [P, P, c_int, c_int, c_int, c_int, P, ctypes.c_double, P, c_ll, P, P],
     "pnp_resample_planes": [P, P, c_int, c_int, c_int, P, c_int, c_int, c_int, c_int, P, P, c_int, P],
     "pnp_native_labels": [P, c_int, c_int, c_int, c_int, P, c_int, c_int, c_int, P, P, P, P],
+    "pnp_largest_components_workspace": [c_int, c_int, c_int, c_int, c_int, P],
+    "pnp_largest_components": [P, c_int, c_int, c_int, c_int, c_int, P, P, P, P, P, c_ll, P],
 }
 
 for _name, _args in SIGNATURES.items():

@@ -1140,6 +1140,57 @@ def native_labels(scores, vmap, shape, gt=None, out=None):
     return out, cm
 
 
+COMPONENT_STATS = ("components", "kept", "removed")
+
+
+def _u8_volume(name, v, shape=None):
+    if not isinstance(v, torch.Tensor) or not v.is_cuda or v.dtype != torch.uint8 or v.dim() != 3:
+        raise ValueError("largest_components: %s must be a uint8 3-D tensor on the device, got %s" % (
+            name, (type(v).__name__ if not isinstance(v, torch.Tensor) else "%s %s on %s" % (v.dtype, tuple(v.shape), v.device))))
+    if shape is not None and tuple(v.shape) != shape:
+        raise ValueError("largest_components: %s must have the labels' shape %s, got %s" % (name, shape, tuple(v.shape)))
+
+
+def largest_components(labels, num_cls, connectivity, gt=None, out=None):
+    """The largest connected component of each class kept, everything else set to background, in one pnp_largest_components
+    call (include/pnp_b200.h, "largest connected component per class").  `labels` uint8 [n0, n1, n2] on the device (labels
+    >= num_cls count as background), `connectivity` 6 (face neighbours) or 26 (face, edge and corner neighbours).  Among
+    components of equal size the one whose first voxel in C order comes first is kept.  Returns (out uint8 [n0, n1, n2] on the
+    device, stats, cm): stats is a dict of host int64 arrays [num_cls] -- `components` (per class, in the input), `kept` and
+    `removed` voxels (index 0: 0, 0 and the number of labels >= num_cls); `gt` uint8 [n0, n1, n2] on the device asks for the
+    confusion counts cm[gt][out] (host int64 [num_cls, num_cls], rows = truth; else None).  `out` may be given to write into,
+    `labels` itself included."""
+    num_cls = int(num_cls)
+    if not 2 <= num_cls <= 8:
+        raise ValueError("largest_components: num_cls must be in [2, 8], got %d" % num_cls)
+    if isinstance(connectivity, bool) or connectivity not in (6, 26):
+        raise ValueError("largest_components: connectivity must be 6 or 26, got %r" % (connectivity,))
+    _u8_volume("labels", labels)
+    shape = tuple(labels.shape)
+    if min(shape) < 1 or labels.numel() >= 1 << 31:
+        raise ValueError("largest_components: every dimension must be >= 1 and the volume below 2^31 voxels, got %s" % (shape,))
+    labels = labels.contiguous()
+    if gt is not None:
+        _u8_volume("gt", gt, shape)
+        gt = gt.contiguous()
+    if out is None:
+        out = torch.empty(shape, dtype=torch.uint8, device=labels.device)
+    else:
+        _u8_volume("out", out, shape)
+        if not out.is_contiguous():
+            raise ValueError("largest_components: out must be contiguous")
+    n0, n1, n2 = shape
+    nbytes = ctypes.c_longlong(0)
+    call("pnp_largest_components_workspace", n0, n1, n2, num_cls, int(connectivity), ctypes.byref(nbytes))
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=labels.device)
+    stats = torch.empty(num_cls, 3, dtype=torch.int64, device=labels.device)
+    cm = None if gt is None else torch.empty(num_cls, num_cls, dtype=torch.int64, device=labels.device)
+    call("pnp_largest_components", ptr(labels), n0, n1, n2, num_cls, int(connectivity), ptr(out), ptr(gt), ptr(cm), ptr(stats),
+         ptr(ws), nbytes.value, rt.stream())
+    st = stats.cpu().numpy()
+    return out, {k: st[:, i].copy() for i, k in enumerate(COMPONENT_STATS)}, (None if cm is None else cm.cpu().numpy())
+
+
 def confusion_counts(logits, y):
     """[C,C] int64 confusion matrix (rows = truth) of argmax(logits) vs one-hot y (lib.py:96-110)."""
     logits, y = logits.contiguous(), y.contiguous()

@@ -14,8 +14,14 @@ for the prepared test split), and a label map of that same scan comes out:
 * scoring against preprocess.map_labels of the native label volume: per-class Dice / Jaccard from the kernel's confusion counts,
   ASSD / HD in mm from functional.surface_distances with the native voxel sizes (the column norms of the image's affine), and
   on request the q-th percentile HD in mm (HD95 at q = 95).
+* optional post-processing (largest_component = 6 or 26): one pnp_largest_components call keeps the largest 3-D connected
+  component of each class and sets the rest to background, in place on the device, before anything else sees the labels; it takes
+  the native ground truth, so Dice / Jaccard come from its counts.  ASSD / HD and the written file are then those of the
+  post-processed labels; the Dice before it (from pnp_native_labels' counts), the number of components and the voxels removed are
+  kept too.
 * outputs under <out>/: native_pred/<name>_label.nii.gz (int16 MMWHS codes 205 / 420 / 500 / 820 for classes 1-4, 0 elsewhere,
-  with the image's shape and affine) and native.csv (one row per subject; <organ>_hd<q>_mm columns when a percentile is asked).
+  with the image's shape and affine) and native.csv (one row per subject; <organ>_hd<q>_mm columns when a percentile is asked,
+  and <organ>_dice_raw / _components / _removed after all the others with the post-processing).
 
 The crop is the ground-truth heart box, as for the prepared test split: a native-grid score is that of a prediction made inside a
 ground-truth region of interest."""
@@ -34,6 +40,8 @@ from .lib import _dice, _jaccard
 from .prepare_data import _upload
 
 CSV_COLUMNS = ("dice", "assd_mm", "hd_mm", "border_pred", "border_gt")
+COMPONENT_COLUMNS = ("dice_raw", "components", "removed")      # per organ, with the largest-component post-processing
+CONNECTIVITIES = (6, 26)
 
 
 def voxel_map(subject):
@@ -122,28 +130,61 @@ def write_prediction(subject, labels, out_dir, num_cls):
     return path
 
 
-def evaluate_subject(logits_fn, image_path, label_path, out_dir, batch_size, num_cls, hd_percentile=None):
-    """one subject end to end -> dict: subject, dice, jaccard, cm, the surface_distances fields, the prediction's path"""
+def check_connectivity(largest_component):
+    """None, or the connectivity 6 or 26 of the largest-component post-processing (ValueError otherwise)"""
+    if largest_component is not None and (isinstance(largest_component, bool) or largest_component not in CONNECTIVITIES):
+        raise ValueError("largest_component must be None, 6 or 26, got %r" % (largest_component,))
+    return None if largest_component is None else int(largest_component)
+
+
+def evaluate_subject(logits_fn, image_path, label_path, out_dir, batch_size, num_cls, hd_percentile=None, largest_component=None):
+    """one subject end to end -> dict: subject, dice, jaccard, cm, the surface_distances fields, the prediction's path.
+    `largest_component` 6 or 26 keeps only the largest connected component of each class of the native labels (in place, before
+    they are scored or written) and adds largest_component, dice_raw (before it), components (in the raw labels), kept and
+    removed (voxels), each [num_cls]."""
+    largest_component = check_connectivity(largest_component)
     s = preprocess.Subject(image_path, label_path)
     scores = predict_scores(s, logits_fn, batch_size, num_cls)
     gt = ground_truth(label_path)
     labels, cm = native_prediction(s, scores, gt)
     del scores
+    post = {}
+    if largest_component is not None:
+        post["dice_raw"] = _dice(cm)
+        labels, stats, cm = F.largest_components(labels, num_cls, largest_component, gt=gt, out=labels)
+        post.update(stats, largest_component=largest_component)
     labels, gt = labels.cpu().numpy(), gt.cpu().numpy()
     res = surface_mm(s, labels, gt, num_cls, hd_percentile)
     res.update(subject=s.name, dice=_dice(cm), jaccard=_jaccard(cm), cm=cm, path=write_prediction(s, labels, out_dir, num_cls))
-    logging.info("%s: native grid %s, %d prepared frames, Dice %s", s.name, s.native_shape, s.D, np.round(res["dice"], 4))
+    res.update(post)
+    if largest_component is None:
+        logging.info("%s: native grid %s, %d prepared frames, Dice %s", s.name, s.native_shape, s.D, np.round(res["dice"], 4))
+    else:
+        logging.info("%s: native grid %s, %d prepared frames, Dice %s (largest %d-connected component; raw Dice %s, %s voxels "
+                     "removed)", s.name, s.native_shape, s.D, np.round(res["dice"], 4), largest_component,
+                     np.round(res["dice_raw"], 4), res["removed"][1:].tolist())
     return res
 
 
+def _largest_component(results):
+    """the connectivity the subjects' dicts carry (None: none); every subject must carry the same"""
+    ks = {r.get("largest_component") for r in results}
+    if len(ks) > 1:
+        raise ValueError("subjects post-processed with different connectivities: %s" % sorted(ks, key=str))
+    return ks.pop() if ks else None
+
+
 def write_csv(path, results, num_cls):
-    """one row per subject: subject, then <organ>_<column> for every organ and CSV_COLUMNS entry (NaN: organ absent), and
-    <organ>_hd<q>_mm when the subjects were scored with a percentile"""
+    """one row per subject: subject, then <organ>_<column> for every organ and CSV_COLUMNS entry (NaN: organ absent),
+    <organ>_hd<q>_mm when the subjects were scored with a percentile, and after all of those <organ>_<column> for every organ and
+    COMPONENT_COLUMNS entry when the labels were post-processed to their largest components"""
     names = evaluation._organ_names(num_cls)
     q = evaluation._hd_percentile(results)
     cols = CSV_COLUMNS if q is None else CSV_COLUMNS + (evaluation.pct_name(q) + "_mm",)
+    post = _largest_component(results) is not None
+    extra = ["%s_%s" % (names[c], k) for c in range(1, num_cls) for k in COMPONENT_COLUMNS] if post else []
     with open(path, "w") as f:
-        f.write(",".join(["subject"] + ["%s_%s" % (names[c], k) for c in range(1, num_cls) for k in cols]) + "\n")
+        f.write(",".join(["subject"] + ["%s_%s" % (names[c], k) for c in range(1, num_cls) for k in cols] + extra) + "\n")
         for r in results:
             row = [str(r["subject"])]
             for c in range(1, num_cls):
@@ -151,17 +192,23 @@ def write_csv(path, results, num_cls):
                         str(int(r["border_gt"][c]))]
                 if q is not None:
                     row.append(repr(float(r["hd_pct"][c])))
+            if post:
+                for c in range(1, num_cls):
+                    row += [repr(float(r["dice_raw"][c])), str(int(r["components"][c])), str(int(r["removed"][c]))]
             f.write(",".join(row) + "\n")
     return path
 
 
-def run(logits_fn, pairs, output_path, batch_size, num_cls, hd_percentile=None):
+def run(logits_fn, pairs, output_path, batch_size, num_cls, hd_percentile=None, largest_component=None):
     """every (image, label) pair through evaluate_subject; writes <output_path>/native_pred/*.nii.gz and native.csv, prints the
     per-organ mean and spread of Dice / Jaccard and of ASSD / HD (and the `hd_percentile`-th percentile HD) in mm -> the
-    per-subject results"""
+    per-subject results.  `largest_component` 6 or 26: every prediction is first reduced to the largest connected component of
+    each class (evaluate_subject); the files and printed figures are then those of the post-processed labels."""
+    largest_component = check_connectivity(largest_component)
     pred_dir = os.path.join(output_path, "native_pred")
     os.makedirs(pred_dir, exist_ok=True)
-    results = [evaluate_subject(logits_fn, im, lb, pred_dir, batch_size, num_cls, hd_percentile) for im, lb in pairs]
+    results = [evaluate_subject(logits_fn, im, lb, pred_dir, batch_size, num_cls, hd_percentile, largest_component)
+               for im, lb in pairs]
     write_csv(os.path.join(output_path, "native.csv"), results, num_cls)
     evaluation.sample_metric_stddev([(r["dice"], r["jaccard"]) for r in results], num_cls)
     evaluation.surface_metric_stddev(results, num_cls, units="mm")
@@ -201,10 +248,14 @@ def main(argv=None):
     ap.add_argument("--batch-size", type=int, default=8, help="frames per forward call")
     ap.add_argument("--hd-percentile", type=float, default=None, metavar="Q",
                     help="also score the Q-th percentile Hausdorff distance in mm (95: HD95; native.csv column <organ>_hd<Q>_mm)")
+    ap.add_argument("--largest-component", type=int, default=None, choices=CONNECTIVITIES, metavar="{6,26}",
+                    help="keep only the largest 6- or 26-connected component of each organ before scoring and writing the "
+                         "prediction (native.csv columns <organ>_dice_raw, _components, _removed)")
     a = ap.parse_args(argv)
     logging.basicConfig(level=logging.INFO)
     trainer = build_trainer(a.trainer, a.checkpoint, a.batch_size)
     os.makedirs(a.out, exist_ok=True)
-    results = trainer.test_native(preprocess.read_pairs(a.pairs), a.out, a.hd_percentile)
+    post = {} if a.largest_component is None else {"largest_component": a.largest_component}
+    results = trainer.test_native(preprocess.read_pairs(a.pairs), a.out, a.hd_percentile, **post)
     print(os.path.join(a.out, "native.csv"))
     return results
