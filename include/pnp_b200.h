@@ -362,6 +362,33 @@ int pnp_surface_distance_pct(const uint8_t* pred, const uint8_t* gt, int n0, int
 int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W, int C,
                         float* img, long long* lab, int label_planes, void* stream);
 
+/* ---- data augmentation: elastic deformation and intensity variation of the resampled planes (resample.cu) ---------------------
+ * pnp_resample_planes_aug is pnp_resample_planes with three optional per-sample fields (device fp32, each may be NULL):
+ *   disp [B][2][H][W]: pixel (r, c) of sample b samples the matrix at (r + d_r, c + d_c), d_r = disp[b][0][r][c],
+ *     d_c = disp[b][1][r][c], each sum rounded (the image and the labels alike, every plane k of the sample);
+ *   gain [B][H][W]: the image value v becomes (1 + gain[b][r][c]) * v;
+ *   ab [B][2]: then a * v + b with (a, b) = (ab[2b], ab[2b + 1]);
+ * out = (a * ((1 + gain) * v)) + b, every operation rounded on its own (no FMA); a NULL field skips its operations.  Every check of
+ * pnp_resample_planes applies; in addition gain or ab without img is PNP_ERR_BAD_ARG and B*2*H*W >= 2^31 with disp is
+ * PNP_ERR_UNSUPPORTED.  With all three NULL the output equals pnp_resample_planes' bit for bit.
+ *
+ * pnp_smooth_noise_field writes out [B][K][H][W] (device fp32) = min(max(amp * s, lo), hi), where s is a uniform field smoothed by a
+ * separable Gaussian:
+ *   x[e] = fl32(w >> 8) * 2^-23 - 1 in [-1, 1) (exact), e = ((b K + k) H + r) W + c, w = 32-bit word e & 3 of Philox4x32-10 block
+ *     e >> 2 with counter (lo(e >> 2), hi(e >> 2), lo(stream_id), hi(stream_id)) and key (lo(seed), hi(seed));
+ *   pass 1 (along c) y[r][c] = sum_{t=-R..R} taps[t + R] * x[r][c + t], pass 2 (along r) s[r][c] = sum_t taps[t + R] * y[r + t][c],
+ *     0 outside the plane, accumulated from +0 in increasing t, every product and every sum rounded on its own (no FMA).
+ * taps (device, 2R + 1 fp32) are typically the normalised Gaussian of scipy.ndimage.gaussian_filter1d (preprocess.gaussian_taps).
+ * tmp (device, B*K*H*W fp32, not out) receives pass 1.  NULL taps / out / tmp, out == tmp, a non-positive size, R < 0, NaN amp or not
+ * lo <= hi are PNP_ERR_BAD_ARG; R > PNP_NF_MAX_R or B*K*H*W >= 2^31 are PNP_ERR_UNSUPPORTED.  On any error nothing is launched and the
+ * outputs are untouched.  Two launches; every output element is written once by one thread, so repeated calls are bit-identical. */
+#define PNP_NF_MAX_R 128
+int pnp_resample_planes_aug(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W, int C,
+                            float* img, long long* lab, int label_planes, const float* disp, const float* gain, const float* ab,
+                            void* stream);
+int pnp_smooth_noise_field(unsigned long long seed, unsigned long long stream_id, int B, int K, int H, int W, const float* taps, int R,
+                           float amp, float lo, float hi, float* out, float* tmp, void* stream);
+
 /* ---- native-grid labels: a prepared-grid prediction sampled back onto the scan's own voxels (resample.cu) ------------------------
  * scores: fp32 C-order [n0][n1][n2][C] class scores on the prepared grid (slice, row, column; C fastest), device.  map: 12 fp32
  * (device) taking native voxel (i, j, k) to the prepared coordinate

@@ -3,7 +3,9 @@
 // of the class-id volume -- straight into the trainers' NHWC layout, so a trainer can draw fresh augmentations every step
 // without record files or a host-to-device image copy.  A grid-stride gather: the writes are coalesced along the NHWC index,
 // the reads follow the sampled coordinates.  The way back (native.py): pnp_native_labels samples the class scores of the prepared
-// grid at every voxel of the subject's native grid with the same taps and lerps, and labels it by their argmax.
+// grid at every voxel of the subject's native grid with the same taps and lerps, and labels it by their argmax.  The opt-in
+// augmentations: pnp_smooth_noise_field draws smoothed Philox noise fields (elastic displacement, bias gain) and
+// pnp_resample_planes_aug resamples at the displaced pixels and applies gain, contrast and offset.
 #include "common.cuh"
 #include "../../include/pnp_b200.h"
 
@@ -35,11 +37,21 @@ __device__ __forceinline__ int axis_nearest(float u, int n) {
   return min((int)floorf(__fadd_rn(u, 0.5f)), n - 1);
 }
 
+// Per-sample augmentation fields of pnp_resample_planes_aug; every pointer may be NULL.  disp [B][2][H][W]: (d_r, d_c) added to
+// the output pixel before its matrix; gain [B][H][W]: g - 1 of the multiplicative bias field; ab [B][2]: contrast a, offset b.
+struct AugFields {
+  const float* disp;
+  const float* gain;
+  const float* ab;
+};
+
 // Item q of the NHWC output: k = q % Cw (or C / 2 when only the middle label plane is written, Cw == 1), pixel = q / Cw.
+// AUG = false is pnp_resample_planes (aug unused); AUG = true is pnp_resample_planes_aug.
+template <bool AUG>
 __global__ void __launch_bounds__(256)
 resample_planes_kernel(const float* __restrict__ vol, const uint8_t* __restrict__ cls, int n0, int n1, int n2,
                        const float* __restrict__ mats, int H, int W, int C, int Cw, long long total, float* __restrict__ img,
-                       long long* __restrict__ lab, int label_planes) {
+                       long long* __restrict__ lab, int label_planes, AugFields aug) {
   pnp_pdl_enter();
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
     const unsigned q = (unsigned)i;
@@ -48,7 +60,12 @@ resample_planes_kernel(const float* __restrict__ vol, const uint8_t* __restrict_
     const unsigned row = pix / (unsigned)W;
     const int c = (int)(pix - row * (unsigned)W), r = (int)(row % (unsigned)H), b = (int)(row / (unsigned)H);
     const float* m = mats + (long long)(b * C + k) * 9;
-    const float fr = (float)r, fc = (float)c;
+    float fr = (float)r, fc = (float)c;
+    if (AUG && aug.disp) {                                  // d_r at b 2HW + r W + c = pix + b HW, d_c one plane later
+      const float* d = aug.disp + (long long)pix + (long long)b * H * W;
+      fr = __fadd_rn(fr, __ldg(d));
+      fc = __fadd_rn(fc, __ldg(d + (long long)H * W));
+    }
     float u[3];
 #pragma unroll
     for (int a = 0; a < 3; ++a) u[a] = __fadd_rn(__fadd_rn(__fmul_rn(__ldg(m + 3 * a), fr), __fmul_rn(__ldg(m + 3 * a + 1), fc)),
@@ -68,7 +85,10 @@ resample_planes_kernel(const float* __restrict__ vol, const uint8_t* __restrict_
       const float v01 = lerp_rn(__ldg(p01 + a2), __ldg(p01 + b2), f2);
       const float v10 = lerp_rn(__ldg(p10 + a2), __ldg(p10 + b2), f2);
       const float v11 = lerp_rn(__ldg(p11 + a2), __ldg(p11 + b2), f2);
-      img[o] = lerp_rn(lerp_rn(v00, v01, f1), lerp_rn(v10, v11, f1), f0);
+      float v = lerp_rn(lerp_rn(v00, v01, f1), lerp_rn(v10, v11, f1), f0);
+      if (AUG && aug.gain) v = __fmul_rn(__fadd_rn(1.f, __ldg(aug.gain + pix)), v);
+      if (AUG && aug.ab) v = __fadd_rn(__fmul_rn(__ldg(aug.ab + 2 * b), v), __ldg(aug.ab + 2 * b + 1));
+      img[o] = v;
     }
     if (label_planes) {
       const int j0 = axis_nearest(u[0], n0), j1 = axis_nearest(u[1], n1), j2 = axis_nearest(u[2], n2);
@@ -141,6 +161,81 @@ native_labels_kernel(const float* __restrict__ scores, int n0, int n1, int n2, i
   }
 }
 
+// ---- smooth noise field (pnp_smooth_noise_field): uniforms on [-1, 1) from Philox, a separable Gaussian along c, then along r
+constexpr int NF_LINE = 256;          // pass 1: outputs per tile, one segment of one row
+constexpr int NF_TC = 32, NF_TR = 64;  // pass 2: a tile of NF_TR rows x NF_TC columns, 256 threads as 8 row groups of 32 columns
+
+// element e of the field: word e & 3 of Philox block e >> 2 of (seed, stream) -> fl32(x >> 8) 2^-23 - 1, exact in fp32
+__device__ __forceinline__ float nf_uniform(unsigned long long seed, unsigned long long stream, unsigned long long e) {
+  const uint4 x = pnp_philox4x32_10(make_uint4((uint32_t)(e >> 2), (uint32_t)(e >> 34), (uint32_t)stream, (uint32_t)(stream >> 32)),
+                                    make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+  const uint32_t w = (e & 2) ? ((e & 1) ? x.w : x.z) : ((e & 1) ? x.y : x.x);
+  return __fsub_rn(__fmul_rn((float)(w >> 8), 0x1p-23f), 1.f);
+}
+
+// s = sum over t = 0 .. n-1 of w[t] x[t * stride], from +0 in increasing t, every product and sum rounded on its own
+__device__ __forceinline__ float nf_taps(const float* ws, const float* x, int n, int stride) {
+  float s = 0.f;
+  for (int t = 0; t < n; ++t) s = __fadd_rn(s, __fmul_rn(ws[t], x[t * stride]));
+  return s;
+}
+
+// pass 1: tile = NF_LINE outputs of one row (line = (b K + k) H + r); the uniforms of the tile and its +-R halo (0 outside the
+// row) are generated into shared memory, so no noise buffer exists.
+__global__ void __launch_bounds__(256)
+noise_field_cols_kernel(unsigned long long seed, unsigned long long stream, int W, const float* __restrict__ taps, int R,
+                        int tiles_per_line, long long tiles, float* __restrict__ tmp) {
+  __shared__ float ws[2 * PNP_NF_MAX_R + 1];
+  __shared__ float xs[NF_LINE + 2 * PNP_NF_MAX_R];
+  pnp_pdl_enter();
+  const int n = 2 * R + 1;
+  for (int t = threadIdx.x; t < n; t += 256) ws[t] = __ldg(taps + t);
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const long long line = tile / tiles_per_line;
+    const int c0 = (int)(tile - line * tiles_per_line) * NF_LINE;
+    __syncthreads();                                       // the previous tile's reads (and the taps) are done
+    for (int i = threadIdx.x; i < NF_LINE + 2 * R; i += 256) {
+      const int c = c0 - R + i;
+      xs[i] = (c >= 0 && c < W) ? nf_uniform(seed, stream, (unsigned long long)(line * W + c)) : 0.f;
+    }
+    __syncthreads();
+    const int c = c0 + (int)threadIdx.x;
+    if (c < W) tmp[line * W + c] = nf_taps(ws, xs + threadIdx.x, n, 1);
+  }
+}
+
+// pass 2: tile = NF_TR rows x NF_TC columns of one plane (b K + k), its rows +-R halo (0 outside the plane) staged in shared
+// memory; out = min(max(amp s, lo), hi)
+__global__ void __launch_bounds__(256)
+noise_field_rows_kernel(const float* __restrict__ tmp, int H, int W, const float* __restrict__ taps, int R, int tiles_r,
+                        int tiles_c, long long tiles, float amp, float lo, float hi, float* __restrict__ out) {
+  __shared__ float ws[2 * PNP_NF_MAX_R + 1];
+  __shared__ float ys[(NF_TR + 2 * PNP_NF_MAX_R) * NF_TC];
+  pnp_pdl_enter();
+  const int n = 2 * R + 1;
+  for (int t = threadIdx.x; t < n; t += 256) ws[t] = __ldg(taps + t);
+  const int tx = threadIdx.x % NF_TC, ty = threadIdx.x / NF_TC;
+  const long long plane_px = (long long)H * W;
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const long long plane = tile / ((long long)tiles_r * tiles_c);
+    const int rest = (int)(tile - plane * tiles_r * tiles_c);
+    const int r0 = (rest / tiles_c) * NF_TR, c0 = (rest % tiles_c) * NF_TC;
+    const float* src = tmp + plane * plane_px;
+    __syncthreads();
+    for (int i = threadIdx.x; i < (NF_TR + 2 * R) * NF_TC; i += 256) {
+      const int r = r0 - R + i / NF_TC, c = c0 + i % NF_TC;
+      ys[i] = (r >= 0 && r < H && c < W) ? src[(long long)r * W + c] : 0.f;
+    }
+    __syncthreads();
+    const int c = c0 + tx;
+    for (int rl = ty; rl < NF_TR; rl += 256 / NF_TC) {
+      const int r = r0 + rl;
+      if (r < H && c < W)
+        out[plane * plane_px + (long long)r * W + c] = fminf(fmaxf(__fmul_rn(amp, nf_taps(ws, ys + rl * NF_TC + tx, n, NF_TC)), lo), hi);
+    }
+  }
+}
+
 // a product of positive ints below 2^31 (each factor is, so no partial product overflows)
 bool count_below_2_31(std::initializer_list<int> dims) {
   long long n = 1;
@@ -151,10 +246,9 @@ bool count_below_2_31(std::initializer_list<int> dims) {
   return true;
 }
 
-}  // namespace
-
-extern "C" int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W,
-                                   int C, float* img, long long* lab, int label_planes, void* stream) {
+// the checks of pnp_resample_planes, shared by pnp_resample_planes_aug
+int check_resample(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W, int C,
+                   const float* img, const long long* lab, int label_planes) {
   if (!mats || n0 <= 0 || n1 <= 0 || n2 <= 0 || B <= 0 || H <= 0 || W <= 0 || C <= 0) return PNP_ERR_BAD_ARG;
   if (label_planes != 0 && label_planes != 1 && label_planes != C) return PNP_ERR_UNSUPPORTED;
   if (!img && !label_planes) return PNP_ERR_BAD_ARG;
@@ -162,10 +256,50 @@ extern "C" int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0,
   if (n0 > PNP_RS_MAX_DIM || n1 > PNP_RS_MAX_DIM || n2 > PNP_RS_MAX_DIM || H > PNP_RS_MAX_DIM || W > PNP_RS_MAX_DIM)
     return PNP_ERR_UNSUPPORTED;
   if (!count_below_2_31({n0, n1, n2}) || !count_below_2_31({B, H, W, C}) || !count_below_2_31({B, C, 9})) return PNP_ERR_UNSUPPORTED;
+  return PNP_OK;
+}
+
+template <bool AUG>
+int launch_resample(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W, int C,
+                    float* img, long long* lab, int label_planes, AugFields aug, void* stream) {
   const int Cw = (img || label_planes != 1) ? C : 1;
   const long long total = (long long)B * H * W * Cw;
-  PNP_CUDA(pnp_launch(resample_planes_kernel, grid_for(total, 256 * 4), 256, 0, (cudaStream_t)stream, vol, cls, n0, n1, n2, mats, H, W,
-                      C, Cw, total, img, lab, label_planes));
+  PNP_CUDA(pnp_launch(resample_planes_kernel<AUG>, grid_for(total, 256 * 4), 256, 0, (cudaStream_t)stream, vol, cls, n0, n1, n2, mats,
+                      H, W, C, Cw, total, img, lab, label_planes, aug));
+  return PNP_OK;
+}
+
+}  // namespace
+
+extern "C" int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W,
+                                   int C, float* img, long long* lab, int label_planes, void* stream) {
+  const int rc = check_resample(vol, cls, n0, n1, n2, mats, B, H, W, C, img, lab, label_planes);
+  if (rc != PNP_OK) return rc;
+  return launch_resample<false>(vol, cls, n0, n1, n2, mats, B, H, W, C, img, lab, label_planes, AugFields{nullptr, nullptr, nullptr},
+                                stream);
+}
+
+extern "C" int pnp_resample_planes_aug(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H,
+                                       int W, int C, float* img, long long* lab, int label_planes, const float* disp,
+                                       const float* gain, const float* ab, void* stream) {
+  const int rc = check_resample(vol, cls, n0, n1, n2, mats, B, H, W, C, img, lab, label_planes);
+  if (rc != PNP_OK) return rc;
+  if (!img && (gain || ab)) return PNP_ERR_BAD_ARG;
+  if (disp && !count_below_2_31({B, 2, H, W})) return PNP_ERR_UNSUPPORTED;
+  return launch_resample<true>(vol, cls, n0, n1, n2, mats, B, H, W, C, img, lab, label_planes, AugFields{disp, gain, ab}, stream);
+}
+
+extern "C" int pnp_smooth_noise_field(unsigned long long seed, unsigned long long stream_id, int B, int K, int H, int W,
+                                      const float* taps, int R, float amp, float lo, float hi, float* out, float* tmp, void* stream) {
+  if (!taps || !out || !tmp || out == tmp || B <= 0 || K <= 0 || H <= 0 || W <= 0 || R < 0) return PNP_ERR_BAD_ARG;
+  if (!(lo <= hi) || !(amp == amp)) return PNP_ERR_BAD_ARG;
+  if (R > PNP_NF_MAX_R || !count_below_2_31({B, K, H, W})) return PNP_ERR_UNSUPPORTED;
+  const int tiles_per_line = pnp_cdiv(W, NF_LINE), tiles_r = pnp_cdiv(H, NF_TR), tiles_c = pnp_cdiv(W, NF_TC);
+  const long long t1 = (long long)B * K * H * tiles_per_line, t2 = (long long)B * K * tiles_r * tiles_c;
+  PNP_CUDA(pnp_launch(noise_field_cols_kernel, grid_for(t1, 1), 256, 0, (cudaStream_t)stream, seed, stream_id, W, taps, R,
+                      tiles_per_line, t1, tmp));
+  PNP_CUDA(pnp_launch(noise_field_rows_kernel, grid_for(t2, 1), 256, 0, (cudaStream_t)stream, (const float*)tmp, H, W, taps, R,
+                      tiles_r, tiles_c, t2, amp, lo, hi, out));
   return PNP_OK;
 }
 

@@ -55,19 +55,32 @@ class VolumeSource:
     to_device is a no-op.  Every subject of `pairs` ((image_path, label_path) NIfTI pairs) is prepared once and its sub-volume
     uploaded; each next() draws per sample a subject, a slice and (augment=True) an augmentation from
     np.random.RandomState(seed), and resamples the whole batch in one pnp_resample_planes launch.  A batch stays valid until
-    the next-but-one call (two alternating output buffers, like TFRecordSource's)."""
+    the next-but-one call (two alternating output buffers, like TFRecordSource's).
 
-    def __init__(self, pairs, batch_size, seed, augment=True):
+    Opt-in augmentations on the device (preprocess.py; both need augment=True):
+    * elastic=True: a displacement field [B, 2, 256, 256] per batch (pnp_smooth_noise_field, Philox stream
+      field_stream(ELASTIC_STREAM_TAG, t)); the subjects are prepared with the reach ELASTIC_REACH_PX;
+    * intensity=True: a bias field [B, 256, 256] (stream field_stream(BIAS_STREAM_TAG, t)) and per sample a contrast and an
+      offset drawn from the generator after that sample's slice and transform.
+    t counts the batches drawn (from 0), so the fields are a function of `seed` alone.  Each field and (a, b) live in buffers of their own
+    for each of the two output buffers; the batch is one pnp_resample_planes_aug launch after the field calls.  With both off
+    nothing extra is drawn or launched, and the batches are those of a source built without the flags."""
+
+    def __init__(self, pairs, batch_size, seed, augment=True, elastic=False, intensity=False):
         from . import preprocess
         from . import runtime as rt
         pairs = list(pairs)
         if not pairs:
             raise ValueError("empty volume list")
-        self.B, self.augment = batch_size, augment
-        self.subjects = [preprocess.Subject(im, lb) for im, lb in pairs]
+        if (elastic or intensity) and not augment:
+            raise ValueError("elastic / intensity augmentation needs augment=True")
+        self.B, self.augment, self.elastic, self.intensity = batch_size, augment, bool(elastic), bool(intensity)
+        reach = preprocess.ELASTIC_REACH_PX if elastic else preprocess.REACH_PX
+        self.subjects = [preprocess.Subject(im, lb, reach_px=reach) for im, lb in pairs]
         vol, cls, self.offsets = preprocess.stack(self.subjects)
         dev = rt.device()
         self.vol, self.cls = torch.from_numpy(vol).to(dev), torch.from_numpy(cls).to(dev)
+        self.seed, self.draws = seed, 0
         self.rng = np.random.RandomState(seed)
         S = preprocess.SIZE
         self._out = [(torch.empty(batch_size, S, S, 3, dtype=torch.float32, device=dev),
@@ -77,28 +90,74 @@ class VolumeSource:
         self._host = [torch.empty(batch_size, 3, 3, 3, dtype=torch.float32, pin_memory=True) for _ in range(2)]
         self._copied = [None, None]
         self._flip = 0
+        self._fields = [{} for _ in range(2)]
+        if elastic or intensity:
+            self._tmp = torch.empty(batch_size * (2 if elastic else 1) * S * S, dtype=torch.float32, device=dev)
+        if elastic:
+            self._elastic_taps = torch.from_numpy(preprocess.gaussian_taps(preprocess.ELASTIC_SIGMA)).to(dev)
+            for f in self._fields:
+                f["disp"] = torch.empty(batch_size, 2, S, S, dtype=torch.float32, device=dev)
+        if intensity:
+            self._bias_taps = torch.from_numpy(preprocess.gaussian_taps(preprocess.BIAS_SIGMA)).to(dev)
+            for f in self._fields:
+                f["gain"] = torch.empty(batch_size, S, S, dtype=torch.float32, device=dev)
+                f["ab"] = torch.empty(batch_size, 2, dtype=torch.float32, device=dev)
+                f["ab_host"] = torch.empty(batch_size, 2, dtype=torch.float32, pin_memory=True)
 
-    def draw_matrices(self):
-        """fp32 [B, 3, 3, 3]: the matrices of the channels j - 1, j, j + 1 of B samples drawn from the generator"""
-        mats = []
+    def draw_samples(self):
+        """(fp32 [B, 3, 3, 3] matrices of the channels j - 1, j, j + 1, fp32 [B, 2] (contrast, offset) or None) of B samples
+        drawn from the generator: per sample the subject, (j, T), then (a, b) when intensity augmentation is on"""
+        from . import preprocess
+        mats, ab = [], []
         for _ in range(self.B):
             s = int(self.rng.randint(len(self.subjects)))
             j, T = self.subjects[s].draw(self.rng, self.augment)
             mats.append(self.subjects[s].matrices((j - 1, j, j + 1), T, self.offsets[s]))
-        return np.stack(mats)
+            if self.intensity:
+                ab.append(preprocess.intensity_draw(self.rng))
+        return np.stack(mats), (np.asarray(ab, np.float64).astype(np.float32) if self.intensity else None)
+
+    def draw_matrices(self):
+        """fp32 [B, 3, 3, 3]: the matrices of the channels j - 1, j, j + 1 of B samples drawn from the generator"""
+        return self.draw_samples()[0]
+
+    def _field(self, tag, t, K, taps, amp, bound, out):
+        from . import preprocess
+        from .functional import smooth_noise_field
+        S = preprocess.SIZE
+        return smooth_noise_field(self.seed, preprocess.field_stream(tag, t), self.B, K, S, S, taps, amp, -bound, bound,
+                                  out=out, tmp=self._tmp[:self.B * K * S * S].view(self.B, K, S, S))
 
     def next(self):
+        from . import preprocess as pp
         from .functional import resample_planes
         i = self._flip
         self._flip ^= 1
         x, y = self._out[i]
+        f = self._fields[i]
         if self._copied[i] is not None:
             self._copied[i].synchronize()
-        self._host[i].numpy()[...] = self.draw_matrices()
+        mats, ab = self.draw_samples()
+        t = self.draws
+        self.draws += 1
+        self._host[i].numpy()[...] = mats
         self._mats[i].copy_(self._host[i], non_blocking=True)
+        if self.intensity:
+            f["ab_host"].numpy()[...] = ab
+            f["ab"].copy_(f["ab_host"], non_blocking=True)
         self._copied[i] = torch.cuda.Event()
         self._copied[i].record()
-        resample_planes(self.vol, self.cls, self._mats[i], x.shape[1], x.shape[2], True, 1, x, y)
+        if not (self.elastic or self.intensity):
+            resample_planes(self.vol, self.cls, self._mats[i], x.shape[1], x.shape[2], True, 1, x, y)
+            return x, y
+        disp = gain = None
+        if self.elastic:
+            disp = self._field(pp.ELASTIC_STREAM_TAG, t, 2, self._elastic_taps, pp.ELASTIC_ALPHA, pp.ELASTIC_MAX_PX, f["disp"])
+        if self.intensity:
+            self._field(pp.BIAS_STREAM_TAG, t, 1, self._bias_taps, pp.BIAS_BETA, pp.BIAS_MAX, f["gain"].view(self.B, 1, *x.shape[1:3]))
+            gain = f["gain"]
+        resample_planes(self.vol, self.cls, self._mats[i], x.shape[1], x.shape[2], True, 1, x, y, disp=disp, gain=gain,
+                        ab=f["ab"] if self.intensity else None)
         return x, y
 
 

@@ -1103,11 +1103,23 @@ def surface_from_raw(raw):
     return res
 
 
-def resample_planes(vol, cls, mats, H, W, image=True, label_planes=1, img=None, lab=None):
+def _aug_field(name, t, shape):
+    if t is None:
+        return None
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or tuple(t.shape) != shape:
+        raise ValueError("resample_planes: %s must be fp32 %s on the device, got %s" % (
+            name, shape, (type(t).__name__ if not isinstance(t, torch.Tensor) else "%s %s on %s" % (t.dtype, tuple(t.shape), t.device))))
+    return t.contiguous()
+
+
+def resample_planes(vol, cls, mats, H, W, image=True, label_planes=1, img=None, lab=None, disp=None, gain=None, ab=None):
     """Planes resampled out of a device volume in one pnp_resample_planes launch (include/pnp_b200.h, "data preparation").
     `vol` fp32 and `cls` uint8 [n0, n1, n2] (either may be None when its output is not wanted), `mats` fp32 [B, C, 3, 3] on the
     device.  Returns (img fp32 [B, H, W, C] or None, lab int64 [B, H, W] (label_planes 1), [B, H, W, C] (label_planes C) or None);
-    `img` / `lab` may be given to write into."""
+    `img` / `lab` may be given to write into.
+    Any of the augmentation fields (fp32 on the device, "data augmentation") makes it one pnp_resample_planes_aug launch: `disp`
+    [B, 2, H, W] displaces each output pixel (r, c) by (d_r, d_c) before its matrix, `gain` [B, H, W] multiplies the image by
+    1 + gain, `ab` [B, 2] then maps it to a * v + b."""
     B, C = mats.shape[0], mats.shape[1]
     ref = vol if vol is not None else cls
     n0, n1, n2 = ref.shape
@@ -1115,9 +1127,34 @@ def resample_planes(vol, cls, mats, H, W, image=True, label_planes=1, img=None, 
         img = torch.empty(B, H, W, C, dtype=torch.float32, device=ref.device)
     if label_planes and lab is None:
         lab = torch.empty((B, H, W) if label_planes == 1 else (B, H, W, C), dtype=torch.int64, device=ref.device)
-    call("pnp_resample_planes", ptr(vol), ptr(cls), n0, n1, n2, ptr(mats), B, H, W, C, ptr(img) if image else None,
-         ptr(lab) if label_planes else None, label_planes, rt.stream())
+    args = (ptr(vol), ptr(cls), n0, n1, n2, ptr(mats), B, H, W, C, ptr(img) if image else None, ptr(lab) if label_planes else None,
+            label_planes)
+    if disp is None and gain is None and ab is None:
+        call("pnp_resample_planes", *args, rt.stream())
+    else:
+        disp, gain, ab = _aug_field("disp", disp, (B, 2, H, W)), _aug_field("gain", gain, (B, H, W)), _aug_field("ab", ab, (B, 2))
+        call("pnp_resample_planes_aug", *args, ptr(disp), ptr(gain), ptr(ab), rt.stream())
     return (img if image else None), (lab if label_planes else None)
+
+
+def smooth_noise_field(seed, stream_id, B, K, H, W, taps, amp, lo, hi, out=None, tmp=None):
+    """A smoothed uniform noise field in one pnp_smooth_noise_field call (two launches; include/pnp_b200.h, "data augmentation"):
+    out [B, K, H, W] = clamp(amp * s, lo, hi), s the Philox uniforms of (seed, stream_id) on [-1, 1) filtered along columns and
+    then rows with `taps` (fp32 [2R + 1] on the device, preprocess.gaussian_taps).  `out` and `tmp` (the first pass, same shape)
+    may be given to write into.  Returns out."""
+    if not isinstance(taps, torch.Tensor) or not taps.is_cuda or taps.dtype != torch.float32 or taps.dim() != 1 or taps.numel() % 2 != 1:
+        raise ValueError("smooth_noise_field: taps must be an odd-length fp32 vector on the device")
+    shape = (B, K, H, W)
+    for name, t in (("out", out), ("tmp", tmp)):
+        if t is not None and (t.dtype != torch.float32 or tuple(t.shape) != shape or not t.is_contiguous()):
+            raise ValueError("smooth_noise_field: %s must be contiguous fp32 %s" % (name, shape))
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=taps.device)
+    if tmp is None:
+        tmp = torch.empty(shape, dtype=torch.float32, device=taps.device)
+    call("pnp_smooth_noise_field", int(seed) & 0xFFFFFFFFFFFFFFFF, int(stream_id) & 0xFFFFFFFFFFFFFFFF, B, K, H, W, ptr(taps),
+         (taps.numel() - 1) // 2, float(amp), float(lo), float(hi), ptr(out), ptr(tmp), rt.stream())
+    return out
 
 
 def native_labels(scores, vmap, shape, gt=None, out=None):

@@ -21,8 +21,17 @@ Host side, in fp64 numpy:
   centre, a scale U(0.9, 1.1) per in-plane axis and a translation U(-10, 10) pixels per axis, from a seeded np.random.RandomState;
   output pixel p samples the un-augmented frame at centre + t + R(theta) S (p - centre).  Matrices are composed in fp64 and
   rounded to fp32 once.  augment=False: the identity at every slice.
+* opt-in augmentations on the device (data.VolumeSource(elastic=, intensity=), prepare_data --elastic / --intensity), fields from
+  functional.smooth_noise_field: uniforms of Philox (seed, field_stream(tag, t)) on [-1, 1) smoothed by gaussian_taps(sigma) along
+  columns, then rows.
+  - elastic: d = clamp(ELASTIC_ALPHA s, +-ELASTIC_MAX_PX) at ELASTIC_SIGMA, per sample, shared by the three channels and the label;
+    output pixel (r, c) samples the matrix at (r + d_r, c + d_c).  Subjects of elastic sources reach ELASTIC_REACH_PX.
+  - intensity: gain g = clamp(1 + BIAS_BETA s, 1 +- BIAS_MAX) at BIAS_SIGMA, then (a, b) = intensity_draw(rng) after the sample's
+    (j, T); image out = a (g v) + b.
+  With both off nothing extra is drawn or launched.
 
-The device side is one pnp_resample_planes launch per batch (functional.resample_planes)."""
+The device side is one pnp_resample_planes launch per batch (functional.resample_planes), plus one pnp_smooth_noise_field call per
+field switched on."""
 import logging
 import math
 import os
@@ -43,6 +52,22 @@ FRAME = ((2, -1), (0, -1), (1, -1))
 CENTRE = (SIZE - 1) / 2.0
 # the farthest an augmented pixel samples from the crop centre, in output pixels
 REACH_PX = SCALE_RANGE[1] * math.hypot(CENTRE, CENTRE) + math.hypot(SHIFT_PX, SHIFT_PX)
+# opt-in elastic deformation: displacement d = clamp(ALPHA s, +-D_MAX) px of a uniform field s smoothed at ELASTIC_SIGMA px
+ELASTIC_SIGMA = 10.0
+ELASTIC_ALPHA = 160.0
+ELASTIC_MAX_PX = 16.0
+# the reach of an elastic source: a displacement of at most D_MAX per axis, through the largest scale
+ELASTIC_REACH_PX = REACH_PX + SCALE_RANGE[1] * math.sqrt(2.0) * ELASTIC_MAX_PX
+# opt-in intensity variation: bias field g = clamp(1 + BIAS_BETA s, 1 +- BIAS_MAX) of a field smoothed at BIAS_SIGMA px, then a
+# contrast a ~ U(CONTRAST_RANGE) and an offset b ~ U(OFFSET_RANGE) (z-score units) per sample
+BIAS_SIGMA = 32.0
+BIAS_BETA = 20.0
+BIAS_MAX = 0.5
+CONTRAST_RANGE = (0.75, 1.25)
+OFFSET_RANGE = (-0.1, 0.1)
+# Philox stream of draw t of a field: tag << 32 | t (dropout streams count up from 1 and stay far below 2^32)
+ELASTIC_STREAM_TAG = 0xE1A5
+BIAS_STREAM_TAG = 0xB1A5
 
 
 def map_labels(raw):
@@ -143,6 +168,29 @@ def augment_transform(rng):
     return T
 
 
+def gaussian_taps(sigma):
+    """fp32 [2R + 1]: the taps of scipy.ndimage.gaussian_filter1d(sigma) (truncate 4, R = int(4 sigma + 0.5)), exp(-t^2 / 2 sigma^2)
+    normalised in fp64 and rounded to fp32 once"""
+    R = int(4.0 * float(sigma) + 0.5)
+    t = np.arange(-R, R + 1, dtype=np.float64)
+    w = np.exp(-0.5 / (float(sigma) * float(sigma)) * t ** 2)
+    return (w / w.sum()).astype(np.float32)
+
+
+def field_stream(tag, t):
+    """the Philox stream of draw t of the field kind `tag` (ELASTIC_STREAM_TAG, BIAS_STREAM_TAG)"""
+    if not 0 <= int(t) < 1 << 32:
+        raise ValueError("field draw index %d outside [0, 2^32)" % t)
+    return (int(tag) << 32) | int(t)
+
+
+def intensity_draw(rng):
+    """one sample's (contrast a, offset b), drawn in that order; only called when intensity augmentation is on"""
+    a = rng.uniform(CONTRAST_RANGE[0], CONTRAST_RANGE[1])
+    b = rng.uniform(OFFSET_RANGE[0], OFFSET_RANGE[1])
+    return a, b
+
+
 def subject_name(image_path):
     b = os.path.basename(str(image_path))
     for ext in (".nii.gz", ".nii"):
@@ -156,7 +204,7 @@ class Subject(object):
     [slice, row, column] of the coronal frame, so a plane's gathers run along contiguous rows.  `D` slices of 256 x 256 pixels of
     `px` mm; the heart covers slices j_lo .. j_hi (each with both neighbours inside the D)."""
 
-    def __init__(self, image_path, label_path, margin=MARGIN):
+    def __init__(self, image_path, label_path, margin=MARGIN, reach_px=REACH_PX):
         self.name = subject_name(image_path)
         im, lb = nifti.load(image_path), nifti.load(label_path)
         if im.shape != lb.shape or len(im.shape) != 3:
@@ -184,8 +232,10 @@ class Subject(object):
             self.j_lo = self.j_hi = min(max(int(round(mid)), 1), D - 2)
         self.p98, self.mu, self.sigma = intensity_stats(raw[box[0][0]:box[0][1] + 1, box[1][0]:box[1][1] + 1,
                                                             box[2][0]:box[2][1] + 1])
-        # the sub-volume every sample can reach: REACH_PX in plane, slices 0 .. D-1, one voxel more for the interpolation
-        reach = np.array([REACH_PX * px / s[0], REACH_PX * px / s[1], mid * px / s[2]])
+        # the sub-volume every sample can reach: reach_px in plane (REACH_PX; ELASTIC_REACH_PX for elastic sources), slices
+        # 0 .. D-1, one voxel more for the interpolation
+        self.reach_px = reach_px
+        reach = np.array([reach_px * px / s[0], reach_px * px / s[1], mid * px / s[2]])
         self.lo = lo = np.floor(c - reach).astype(np.int64) - 1
         hi = np.ceil(c + reach).astype(np.int64) + 1
         idx = [np.arange(lo[a], hi[a] + 1) for a in range(3)]

@@ -66,9 +66,15 @@ def main(phase, argv=None):
     ap.add_argument("--synthetic", action="store_true", help="ignore the list files and train on the synthetic sources")
     ap.add_argument("--volumes", action="store_true",
                     help="draw freshly augmented slices on the GPU from the NIfTI pairs of <lists>/{mr,ct}_{train,val}_volumes")
+    ap.add_argument("--elastic", action="store_true",
+                    help="with --volumes: add smooth random elastic deformations to the MR and CT training slices (preprocess.py)")
+    ap.add_argument("--intensity", action="store_true",
+                    help="with --volumes: add a smooth bias field, a contrast and an offset to the MR and CT training slices")
     ap.add_argument("--image-summaries", action="store_true",
                     help="also write the reference's TensorBoard image summaries (prediction, input slice, ground truth) every display step")
     a = ap.parse_args(argv)
+    if (a.elastic or a.intensity) and not a.volumes:
+        ap.error("--elastic / --intensity augment the slices drawn with --volumes; give --volumes")
     logging.basicConfig(level=logging.INFO)
     parallel.init_from_env()
     if a.conv_backend:
@@ -88,9 +94,11 @@ def main(phase, argv=None):
         # each stream keeps the seed of the stream it replaces (adversarial.Trainer.train: 1234 / 4321 / 2234 / 5321 + rank)
         from .train_segmenter import volume_source
         rank = parallel.DataParallel().rank
-        for key, name, seed in (("mr_source", "mr_train_volumes", 1234), ("ct_source", "ct_train_volumes", 4321),
-                                ("mr_val_source", "mr_val_volumes", 2234), ("ct_val_source", "ct_val_volumes", 5321)):
-            sources[key] = volume_source(os.path.join(a.lists, name), a.batch_size, seed + rank)
+        # the opt-in augmentations apply to the two training streams only
+        aug = {"elastic": a.elastic, "intensity": a.intensity}
+        for key, name, seed, kw in (("mr_source", "mr_train_volumes", 1234, aug), ("ct_source", "ct_train_volumes", 4321, aug),
+                                    ("mr_val_source", "mr_val_volumes", 2234, {}), ("ct_val_source", "ct_val_volumes", 5321, {})):
+            sources[key] = volume_source(os.path.join(a.lists, name), a.batch_size, seed + rank, **kw)
     trainer = drn.Trainer(net, mr_train, mr_val, ct_train, ct_val, num_cls=num_cls, batch_size=a.batch_size,
                           opt_kwargs=dict(opt_kwargs), train_config=tc, **sources)
     print("Now start training...")

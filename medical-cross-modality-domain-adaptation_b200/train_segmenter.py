@@ -43,13 +43,13 @@ def resolve_lists(*fids_and_flag):
     return out
 
 
-def volume_source(pairs_file, batch_size, seed):
-    """data.VolumeSource over the `image label` pairs of a list file"""
+def volume_source(pairs_file, batch_size, seed, elastic=False, intensity=False):
+    """data.VolumeSource over the `image label` pairs of a list file (elastic / intensity: its opt-in augmentations)"""
     from .data import VolumeSource
     from .preprocess import read_pairs
     pairs = read_pairs(pairs_file)
     logging.info("%s: %d volume pairs" % (pairs_file, len(pairs)))
-    return VolumeSource(pairs, batch_size, seed)
+    return VolumeSource(pairs, batch_size, seed, elastic=elastic, intensity=intensity)
 
 
 def main(argv=None):
@@ -66,9 +66,15 @@ def main(argv=None):
     ap.add_argument("--train-volumes", default=None,
                     help="file of `image label` NIfTI pairs: draw freshly augmented training slices from these volumes on the GPU")
     ap.add_argument("--val-volumes", default=None, help="file of `image label` NIfTI pairs: validation slices from these volumes")
+    ap.add_argument("--elastic", action="store_true",
+                    help="with --train-volumes: add smooth random elastic deformations to the training slices (preprocess.py)")
+    ap.add_argument("--intensity", action="store_true",
+                    help="with --train-volumes: add a smooth bias field, a contrast and an offset to the training slices")
     ap.add_argument("--image-summaries", action="store_true",
                     help="also write the reference's TensorBoard image summaries (prediction, input slice, ground truth) every display step")
     a = ap.parse_args(argv)
+    if (a.elastic or a.intensity) and not a.train_volumes:
+        ap.error("--elastic / --intensity augment the slices drawn from --train-volumes; give --train-volumes")
     logging.basicConfig(level=logging.INFO)
     parallel.init_from_env()
     if a.conv_backend:
@@ -77,8 +83,11 @@ def main(argv=None):
     print("Network has been built ...")
     train_list, val_list = resolve_lists(a.train_list, a.val_list, a.synthetic)
     # VolumeSource streams take the seeds of the streams they replace (source_segmenter.Trainer.train: 1234 / 4321 + rank)
-    sources = {k: volume_source(path, a.batch_size, seed + parallel.DataParallel().rank) for k, path, seed in
-               (("source", a.train_volumes, 1234), ("val_source", a.val_volumes, 4321)) if path}
+    # the opt-in augmentations apply to the training stream only
+    rank = parallel.DataParallel().rank
+    sources = {k: volume_source(path, a.batch_size, seed + rank, **aug) for k, path, seed, aug in
+               (("source", a.train_volumes, 1234, {"elastic": a.elastic, "intensity": a.intensity}),
+                ("val_source", a.val_volumes, 4321, {})) if path}
     trainer = drn.Trainer(net, train_list=train_list, val_list=val_list, num_cls=num_cls, batch_size=a.batch_size, opt_kwargs=dict(opt_kwargs),
                           checkpoint_space=checkpoint_space, optimizer=optimizer, lr_update_flag=False, **sources)
     print("Now start training...")
