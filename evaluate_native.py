@@ -1,6 +1,9 @@
-"""python evaluate_native.py --trainer gan|segmenter --checkpoint CKPT.npz --pairs LIST --out DIR [--batch-size B]
-[--hd-percentile Q] -- segment raw MMWHS subjects on their own voxel grid and score them there in mm (native.py):
-DIR/native_pred/<name>_label.nii.gz and DIR/native.csv (with <organ>_hd<Q>_mm columns when Q is given, e.g. hd95_mm)."""
+"""python evaluate_native.py --trainer gan|segmenter --checkpoint CKPT.npz [CKPT2.npz ...] --pairs LIST --out DIR [--batch-size B]
+[--hd-percentile Q] [--largest-component 6|26] [--tta-rotations DEG ...] [--tta-scales S ...] -- segment raw MMWHS subjects on
+their own voxel grid and score them there in mm (native.py): DIR/native_pred/<name>_label.nii.gz and DIR/native.csv (with
+<organ>_hd<Q>_mm columns when Q is given, e.g. hd95_mm).  Several checkpoints and / or test-time rotations and scales are
+ensembled: their class probabilities are summed at every native voxel before the argmax (native.csv adds members and
+<organ>_dice_first)."""
 from pnp_b200.native import main
 
 if __name__ == "__main__":

@@ -405,6 +405,25 @@ int pnp_smooth_noise_field(unsigned long long seed, unsigned long long stream_id
 int pnp_native_labels(const float* scores, int n0, int n1, int n2, int C, const float* map, int m0, int m1, int m2, uint8_t* out,
                       const uint8_t* gt, long long* cm, void* stream);
 
+/* ---- native-grid labels of an ensemble: K predictions averaged at every native voxel before the argmax (resample.cu) ----------
+ * Checkpoint ensembles and test-time augmentation.  scores: fp32 C-order [K][n0][n1][n2][C] on the device, one prepared-grid score
+ * volume per member, all of one shape (member k starts at k * n0*n1*n2*C, a 64-bit offset).  maps: fp32 [K][12] on the device,
+ * member k's map in pnp_native_labels' layout.  For every native voxel, in ascending k: u^k is computed as pnp_native_labels
+ * computes it; member k covers the voxel when every u^k_a is inside [-0.5, n_a - 0.5) and not NaN; its class scores v^k_c are
+ * pnp_native_labels' trilinear scores.  The first covering member's scores are taken as they are, each later covering member's
+ * are added to them (fp32, each sum rounded, ascending k).
+ *   out (uint8): the first maximum over c (the lowest index wins a tie) of the sums; 0 where no member covers the voxel.  The sum
+ *     is not divided by the number of covering members: every class shares that number, and a division could create a tie.  At
+ *     K = 1 out and cm are pnp_native_labels' bit for bit.
+ *   cm: as pnp_native_labels counts it.
+ * K <= 0 or NULL maps, and every argument pnp_native_labels rejects as PNP_ERR_BAD_ARG, are PNP_ERR_BAD_ARG; K above
+ * PNP_NATIVE_MAX_MEMBERS (the maps are staged in shared memory once per CTA), and each member outside pnp_native_labels' limits,
+ * are PNP_ERR_UNSUPPORTED.  On any error nothing is launched and the outputs are untouched.  Every label is written once by one
+ * thread and the counts are integers, so repeated calls are bit-identical. */
+#define PNP_NATIVE_MAX_MEMBERS 16
+int pnp_native_labels_ensemble(const float* scores, int K, int n0, int n1, int n2, int C, const float* maps, int m0, int m1, int m2,
+                               uint8_t* out, const uint8_t* gt, long long* cm, void* stream);
+
 /* ---- evaluation: largest connected component per class (components3d.cu) ------------------------------------------------------
  * The usual clean-up of a segmentation (nnU-Net's post-processing): every structure is one connected body, so only the largest
  * 3-D connected component of each class is kept and the rest is set to background.  labels, out and gt are uint8 C-order

@@ -3,7 +3,8 @@
 // of the class-id volume -- straight into the trainers' NHWC layout, so a trainer can draw fresh augmentations every step
 // without record files or a host-to-device image copy.  A grid-stride gather: the writes are coalesced along the NHWC index,
 // the reads follow the sampled coordinates.  The way back (native.py): pnp_native_labels samples the class scores of the prepared
-// grid at every voxel of the subject's native grid with the same taps and lerps, and labels it by their argmax.  The opt-in
+// grid at every voxel of the subject's native grid with the same taps and lerps, and labels it by their argmax;
+// pnp_native_labels_ensemble sums the scores of several members (checkpoints, test-time transforms) first.  The opt-in
 // augmentations: pnp_smooth_noise_field draws smoothed Philox noise fields (elastic displacement, bias gain) and
 // pnp_resample_planes_aug resamples at the displaced pixels and applies gain, contrast and offset.
 #include "common.cuh"
@@ -101,48 +102,81 @@ resample_planes_kernel(const float* __restrict__ vol, const uint8_t* __restrict_
 
 // Native voxel q = (i m1 + j) m2 + k: trilinear class scores at its prepared-grid coordinate, first-max argmax, and with gt the
 // (truth, prediction) pair in a per-CTA histogram flushed by one global atomic per non-zero bin.
+// ENS = false is pnp_native_labels: one member, its map held in registers (K and stride unused).
+// ENS = true is pnp_native_labels_ensemble: member k's scores start at scores + k stride and its map at map + 12 k; the maps are
+// staged in shared memory once per CTA, and the class scores of the members covering the voxel are summed in ascending k (the
+// first one taken as it is) before the argmax.
+template <bool ENS>
 __global__ void __launch_bounds__(256)
 native_labels_kernel(const float* __restrict__ scores, int n0, int n1, int n2, int C, const float* __restrict__ map, int m1, int m2,
-                     long long total, uint8_t* __restrict__ out, const uint8_t* __restrict__ gt, long long* __restrict__ cm) {
+                     long long total, uint8_t* __restrict__ out, const uint8_t* __restrict__ gt, long long* __restrict__ cm, int K,
+                     long long stride) {
   __shared__ unsigned int hist[64];
+  __shared__ float maps[ENS ? 12 * PNP_NATIVE_MAX_MEMBERS : 1];
   pnp_pdl_enter();
   if (cm) {
     if (threadIdx.x < 64) hist[threadIdx.x] = 0u;
     __syncthreads();
   }
   float m[12];
+  if (ENS) {
+    if (threadIdx.x < 12 * K) maps[threadIdx.x] = __ldg(map + threadIdx.x);
+    __syncthreads();
+  } else {
 #pragma unroll
-  for (int t = 0; t < 12; ++t) m[t] = __ldg(map + t);
+    for (int t = 0; t < 12; ++t) m[t] = __ldg(map + t);
+  }
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
     const unsigned q = (unsigned)i;
     const unsigned row = q / (unsigned)m2;
     const float fk = (float)(q - row * (unsigned)m2), fj = (float)(row % (unsigned)m1), fi = (float)(row / (unsigned)m1);
-    float u[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-      u[a] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[4 * a], fi), __fmul_rn(m[4 * a + 1], fj)), __fmul_rn(m[4 * a + 2], fk)),
-                       m[4 * a + 3]);
     int best = 0;
-    if (axis_inside(u[0], n0) && axis_inside(u[1], n1) && axis_inside(u[2], n2)) {
-      int a0, b0, a1, b1, a2, b2;
-      float f0, f1, f2;
-      axis_taps(u[0], n0, a0, b0, f0);
-      axis_taps(u[1], n1, a1, b1, f1);
-      axis_taps(u[2], n2, a2, b2, f2);
-      const float* p00 = scores + (long long)((a0 * n1 + a1) * n2) * C;
-      const float* p01 = scores + (long long)((a0 * n1 + b1) * n2) * C;
-      const float* p10 = scores + (long long)((b0 * n1 + a1) * n2) * C;
-      const float* p11 = scores + (long long)((b0 * n1 + b1) * n2) * C;
-      const int o0 = a2 * C, o1 = b2 * C;
-      float top = 0.f;
-      for (int c = 0; c < C; ++c) {
-        const float v00 = lerp_rn(__ldg(p00 + o0 + c), __ldg(p00 + o1 + c), f2);
-        const float v01 = lerp_rn(__ldg(p01 + o0 + c), __ldg(p01 + o1 + c), f2);
-        const float v10 = lerp_rn(__ldg(p10 + o0 + c), __ldg(p10 + o1 + c), f2);
-        const float v11 = lerp_rn(__ldg(p11 + o0 + c), __ldg(p11 + o1 + c), f2);
-        const float v = lerp_rn(lerp_rn(v00, v01, f1), lerp_rn(v10, v11, f1), f0);
-        if (c == 0 || v > top) {       // strictly greater: the lowest index wins a tie
-          top = v;
+    float sum[8];                        // ENS: the summed class scores (C <= 8, fully unrolled: they stay in registers)
+    bool covered = false;                // ENS: some member covers the voxel
+    for (int e = 0; e < (ENS ? K : 1); ++e) {
+      const float* mk = ENS ? maps + 12 * e : m;
+      const float* member = ENS ? scores + (long long)e * stride : scores;
+      float u[3];
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+        u[a] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(mk[4 * a], fi), __fmul_rn(mk[4 * a + 1], fj)), __fmul_rn(mk[4 * a + 2], fk)),
+                         mk[4 * a + 3]);
+      if (axis_inside(u[0], n0) && axis_inside(u[1], n1) && axis_inside(u[2], n2)) {
+        int a0, b0, a1, b1, a2, b2;
+        float f0, f1, f2;
+        axis_taps(u[0], n0, a0, b0, f0);
+        axis_taps(u[1], n1, a1, b1, f1);
+        axis_taps(u[2], n2, a2, b2, f2);
+        const float* p00 = member + (long long)((a0 * n1 + a1) * n2) * C;
+        const float* p01 = member + (long long)((a0 * n1 + b1) * n2) * C;
+        const float* p10 = member + (long long)((b0 * n1 + a1) * n2) * C;
+        const float* p11 = member + (long long)((b0 * n1 + b1) * n2) * C;
+        const int o0 = a2 * C, o1 = b2 * C;
+        float top = 0.f;
+#pragma unroll
+        for (int c = 0; c < (ENS ? 8 : C); ++c) {     // ENS unrolls to 8 classes and stops at C
+          if (ENS && c >= C) break;
+          const float v00 = lerp_rn(__ldg(p00 + o0 + c), __ldg(p00 + o1 + c), f2);
+          const float v01 = lerp_rn(__ldg(p01 + o0 + c), __ldg(p01 + o1 + c), f2);
+          const float v10 = lerp_rn(__ldg(p10 + o0 + c), __ldg(p10 + o1 + c), f2);
+          const float v11 = lerp_rn(__ldg(p11 + o0 + c), __ldg(p11 + o1 + c), f2);
+          const float v = lerp_rn(lerp_rn(v00, v01, f1), lerp_rn(v10, v11, f1), f0);
+          if (ENS) {
+            sum[c] = covered ? __fadd_rn(sum[c], v) : v;     // the first covering member is taken as it is
+          } else if (c == 0 || v > top) {       // strictly greater: the lowest index wins a tie
+            top = v;
+            best = c;
+          }
+        }
+        covered = true;
+      }
+    }
+    if (ENS && covered) {
+      float top = sum[0];
+#pragma unroll
+      for (int c = 1; c < 8; ++c) {
+        if (c < C && sum[c] > top) {     // strictly greater: the lowest index wins a tie
+          top = sum[c];
           best = c;
         }
       }
@@ -269,6 +303,30 @@ int launch_resample(const float* vol, const uint8_t* cls, int n0, int n1, int n2
   return PNP_OK;
 }
 
+// the checks of pnp_native_labels, shared by pnp_native_labels_ensemble (whose every member has the shape n0 x n1 x n2 x C)
+int check_native(const float* scores, int n0, int n1, int n2, int C, const float* map, int m0, int m1, int m2, const uint8_t* out,
+                 const uint8_t* gt, const long long* cm) {
+  if (!scores || !map || !out || (!gt) != (!cm) || n0 <= 0 || n1 <= 0 || n2 <= 0 || m0 <= 0 || m1 <= 0 || m2 <= 0)
+    return PNP_ERR_BAD_ARG;
+  if (C < 2 || C > 8) return PNP_ERR_UNSUPPORTED;
+  if (n0 > PNP_RS_MAX_DIM || n1 > PNP_RS_MAX_DIM || n2 > PNP_RS_MAX_DIM || m0 > PNP_RS_MAX_DIM || m1 > PNP_RS_MAX_DIM ||
+      m2 > PNP_RS_MAX_DIM)
+    return PNP_ERR_UNSUPPORTED;
+  if (!count_below_2_31({n0, n1, n2, C}) || !count_below_2_31({m0, m1, m2})) return PNP_ERR_UNSUPPORTED;
+  return PNP_OK;
+}
+
+template <bool ENS>
+int launch_native(const float* scores, int K, int n0, int n1, int n2, int C, const float* map, int m0, int m1, int m2, uint8_t* out,
+                  const uint8_t* gt, long long* cm, void* stream) {
+  const long long total = (long long)m0 * m1 * m2;
+  const long long stride = (long long)n0 * n1 * n2 * C;
+  if (cm) PNP_CUDA(cudaMemsetAsync(cm, 0, sizeof(long long) * C * C, (cudaStream_t)stream));
+  PNP_CUDA(pnp_launch(native_labels_kernel<ENS>, grid_for(total, 256 * 4), 256, 0, (cudaStream_t)stream, scores, n0, n1, n2, C, map,
+                      m1, m2, total, out, gt, cm, K, stride));
+  return PNP_OK;
+}
+
 }  // namespace
 
 extern "C" int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W,
@@ -305,16 +363,16 @@ extern "C" int pnp_smooth_noise_field(unsigned long long seed, unsigned long lon
 
 extern "C" int pnp_native_labels(const float* scores, int n0, int n1, int n2, int C, const float* map, int m0, int m1, int m2,
                                  uint8_t* out, const uint8_t* gt, long long* cm, void* stream) {
-  if (!scores || !map || !out || (!gt) != (!cm) || n0 <= 0 || n1 <= 0 || n2 <= 0 || m0 <= 0 || m1 <= 0 || m2 <= 0)
-    return PNP_ERR_BAD_ARG;
-  if (C < 2 || C > 8) return PNP_ERR_UNSUPPORTED;
-  if (n0 > PNP_RS_MAX_DIM || n1 > PNP_RS_MAX_DIM || n2 > PNP_RS_MAX_DIM || m0 > PNP_RS_MAX_DIM || m1 > PNP_RS_MAX_DIM ||
-      m2 > PNP_RS_MAX_DIM)
-    return PNP_ERR_UNSUPPORTED;
-  if (!count_below_2_31({n0, n1, n2, C}) || !count_below_2_31({m0, m1, m2})) return PNP_ERR_UNSUPPORTED;
-  const long long total = (long long)m0 * m1 * m2;
-  if (cm) PNP_CUDA(cudaMemsetAsync(cm, 0, sizeof(long long) * C * C, (cudaStream_t)stream));
-  PNP_CUDA(pnp_launch(native_labels_kernel, grid_for(total, 256 * 4), 256, 0, (cudaStream_t)stream, scores, n0, n1, n2, C, map, m1,
-                      m2, total, out, gt, cm));
-  return PNP_OK;
+  const int rc = check_native(scores, n0, n1, n2, C, map, m0, m1, m2, out, gt, cm);
+  if (rc != PNP_OK) return rc;
+  return launch_native<false>(scores, 1, n0, n1, n2, C, map, m0, m1, m2, out, gt, cm, stream);
+}
+
+extern "C" int pnp_native_labels_ensemble(const float* scores, int K, int n0, int n1, int n2, int C, const float* maps, int m0, int m1,
+                                          int m2, uint8_t* out, const uint8_t* gt, long long* cm, void* stream) {
+  if (K <= 0 || !maps) return PNP_ERR_BAD_ARG;
+  const int rc = check_native(scores, n0, n1, n2, C, maps, m0, m1, m2, out, gt, cm);
+  if (rc != PNP_OK) return rc;
+  if (K > PNP_NATIVE_MAX_MEMBERS) return PNP_ERR_UNSUPPORTED;
+  return launch_native<true>(scores, K, n0, n1, n2, C, maps, m0, m1, m2, out, gt, cm, stream);
 }

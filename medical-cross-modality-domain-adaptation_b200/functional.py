@@ -1161,9 +1161,18 @@ def native_labels(scores, vmap, shape, gt=None, out=None):
     """A prepared-grid prediction sampled back onto a native grid in one pnp_native_labels launch (include/pnp_b200.h,
     "native-grid labels").  `scores` fp32 [n0, n1, n2, C] on the device, `vmap` fp32 [12] (device) from native voxel to prepared
     coordinate, `shape` the native (m0, m1, m2).  Returns (labels uint8 [m0, m1, m2], confusion counts int64 [C, C] (rows =
-    truth) or None); `gt` uint8 [m0, m1, m2] on the device asks for the counts, `out` may be given to write into."""
+    truth) or None); `gt` uint8 [m0, m1, m2] on the device asks for the counts, `out` may be given to write into.
+    An ensemble -- `scores` fp32 [K, n0, n1, n2, C] with `vmap` fp32 [K, 12], member k's scores and map -- is one
+    pnp_native_labels_ensemble launch: the class scores of the members covering each native voxel are summed in ascending k
+    before the argmax ("native-grid labels of an ensemble")."""
     scores, vmap = scores.contiguous(), vmap.contiguous()
-    n0, n1, n2, C = scores.shape
+    if scores.dim() == 5:
+        K, n0, n1, n2, C = scores.shape
+        if tuple(vmap.shape) != (K, 12):
+            raise ValueError("native_labels: an ensemble of %d members needs vmap [%d, 12], got %s" % (K, K, tuple(vmap.shape)))
+    else:
+        K = None
+        n0, n1, n2, C = scores.shape
     m0, m1, m2 = (int(s) for s in shape)
     if out is None:
         out = torch.empty(m0, m1, m2, dtype=torch.uint8, device=scores.device)
@@ -1173,7 +1182,11 @@ def native_labels(scores, vmap, shape, gt=None, out=None):
         if tuple(gt.shape) != (m0, m1, m2) or gt.dtype != torch.uint8:
             raise ValueError("native_labels: gt must be uint8 %s, got %s %s" % ((m0, m1, m2), tuple(gt.shape), gt.dtype))
         cm = torch.empty(C, C, dtype=torch.int64, device=scores.device)
-    call("pnp_native_labels", ptr(scores), n0, n1, n2, C, ptr(vmap), m0, m1, m2, ptr(out), ptr(gt), ptr(cm), rt.stream())
+    if K is None:
+        call("pnp_native_labels", ptr(scores), n0, n1, n2, C, ptr(vmap), m0, m1, m2, ptr(out), ptr(gt), ptr(cm), rt.stream())
+    else:
+        call("pnp_native_labels_ensemble", ptr(scores), K, n0, n1, n2, C, ptr(vmap), m0, m1, m2, ptr(out), ptr(gt), ptr(cm),
+             rt.stream())
     return out, cm
 
 

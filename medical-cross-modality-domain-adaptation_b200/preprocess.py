@@ -157,10 +157,26 @@ def intensity_stats(raw_box):
 
 def augment_transform(rng):
     """a 3 x 3 fp64 map from output pixel (r, c, 1) to the un-augmented frame: rotation, per-axis scale, translation (drawn in
-    that order)"""
-    th = np.deg2rad(rng.uniform(-ROTATION_DEG, ROTATION_DEG))
+    that order; tta_transform composes them)"""
+    th = rng.uniform(-ROTATION_DEG, ROTATION_DEG)
     s = rng.uniform(SCALE_RANGE[0], SCALE_RANGE[1], 2)
     t = rng.uniform(-SHIFT_PX, SHIFT_PX, 2)
+    return tta_transform(th, s, t)
+
+
+def tta_transform(theta_deg, scale=(1.0, 1.0), shift=(0.0, 0.0)):
+    """the deterministic form of augment_transform: a 3 x 3 fp64 map from output pixel (r, c, 1) to the un-augmented frame,
+    centre + t + R(theta) diag(s) (p - centre), for a rotation of `theta_deg` degrees, per-axis scale (s_r, s_c) and translation
+    (t_r, t_c) in pixels.  Values outside the training ranges (ROTATION_DEG, SCALE_RANGE, SHIFT_PX) raise ValueError: the network
+    has not seen such transforms, and the uploaded sub-volume only reaches REACH_PX."""
+    s, t = np.asarray(scale, np.float64).reshape(2), np.asarray(shift, np.float64).reshape(2)
+    if not -ROTATION_DEG <= float(theta_deg) <= ROTATION_DEG:
+        raise ValueError("rotation %r degrees outside the training range [-%g, %g]" % (theta_deg, ROTATION_DEG, ROTATION_DEG))
+    if not all(SCALE_RANGE[0] <= float(x) <= SCALE_RANGE[1] for x in s):
+        raise ValueError("scale %s outside the training range [%g, %g]" % (s.tolist(), SCALE_RANGE[0], SCALE_RANGE[1]))
+    if not all(-SHIFT_PX <= float(x) <= SHIFT_PX for x in t):
+        raise ValueError("shift %s px outside the training range [-%g, %g]" % (t.tolist(), SHIFT_PX, SHIFT_PX))
+    th = np.deg2rad(theta_deg)
     A = np.array([[math.cos(th), -math.sin(th)], [math.sin(th), math.cos(th)]]) @ np.diag(s)
     T = np.eye(3)
     T[:2, :2] = A
