@@ -294,6 +294,25 @@ int pnp_momentum_step(float* theta, const float* grad, float* accum, long long n
                       const float* lr_ptr, float momentum, float grad_scale, void* stream);
 int pnp_fill(float* p, float v, long long n, void* stream);
 
+/* ---- exponential moving average of the trained weights (tf.train.ExponentialMovingAverage(decay, num_updates=n)) --------------
+ * Every operation is fp32 and rounded on its own (no FMA contraction):
+ *   pnp_ema_advance: nf = (float)n; d = fminf(decay, (1 + nf) / (10 + nf)); *c = 1 - d; n += 1.  One thread; n (int64) and c
+ *                    live in device memory, so a captured graph advances the schedule on every replay.  0 < decay < 1.
+ *   pnp_ema_update:  s = s - (s - x) * c for every covered float (assign_moving_average's assign_sub form), c read from device.
+ *   pnp_ema_swap:    exchanges s and x.
+ * The shadow is one flat buffer of arena_n + 1024 * table_n floats.  Its first arena_n floats (a multiple of 1024) mirror the
+ * live optimizer arena float for float, padding included.  Each of the table_n chunks that follow belongs to one entry of
+ * `table` (device memory): `len` (1..1024) live floats from `live`, the rest of the chunk is padding nobody touches.  A tensor
+ * longer than 1024 floats takes ceil(len / 1024) consecutive entries.  One CTA per 1024-float chunk. */
+typedef struct {
+  float* live;
+  long long len;
+} pnp_ema_chunk;
+int pnp_ema_advance(long long* num_updates, float decay, float* c, void* stream);
+int pnp_ema_update(float* shadow, const float* arena, long long arena_n, const pnp_ema_chunk* table, int table_n, const float* c,
+                   void* stream);
+int pnp_ema_swap(float* shadow, float* arena, long long arena_n, const pnp_ema_chunk* table, int table_n, void* stream);
+
 /* ---- evaluation: 3-D surface distances ---------------------------------------------------------------------------------------
  * Per-class surface distances between a predicted label volume P and a ground truth G (medpy.metric.binary.assd / hd as the
  * papers' evaluation calls them).  pred and gt are uint8 [n0][n1][n2] (n2 fastest) on the device; labels >= C count as

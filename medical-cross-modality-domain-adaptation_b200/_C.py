@@ -101,6 +101,9 @@ SIGNATURES = {
     "pnp_rmsprop_step": [P, P, P, P, c_ll, P, P, P, P, c_float, c_float, c_float, c_float, P],
     "pnp_momentum_step": [P, P, P, c_ll, P, P, P, c_float, c_float, P],
     "pnp_fill": [P, c_float, c_ll, P],
+    "pnp_ema_advance": [P, c_float, P, P],
+    "pnp_ema_update": [P, P, c_ll, P, c_int, P, P],
+    "pnp_ema_swap": [P, P, c_ll, P, c_int, P],
     "pnp_surface_distance_workspace": [c_int, c_int, c_int, c_int, P],
     "pnp_surface_distance": [P, P, c_int, c_int, c_int, c_int, P, P, c_ll, P, P],
     "pnp_surface_distance_pct_workspace": [c_int, c_int, c_int, c_int, P],

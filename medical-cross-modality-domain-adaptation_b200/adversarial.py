@@ -28,6 +28,7 @@ from . import parallel
 from . import runtime as rt
 from . import summary
 from .data import pick_source, to_device
+from .ema import EMA
 from .lib import save_checkpoint
 from .networks import FB, FRONT, BACK, SegmenterHalf, SegmenterTail
 
@@ -320,7 +321,10 @@ class Trainer(object):
     def __init__(self, net, mr_train_list=None, mr_val_list=None, ct_train_list=None, ct_val_list=None, adapt_var_list=None,
                  mr_var_list=None, old_bn_list=None, new_bn_list=None, test_label_list=None, test_nii_list=None, num_cls=None,
                  batch_size=6, opt_kwargs={}, train_config={}, mr_source=None, ct_source=None, mr_val_source=None,
-                 ct_val_source=None):
+                 ct_val_source=None, ema_decay=None):
+        """`ema_decay`: keep an exponential moving average (ema.EMA) of every adapt_* variable -- the G arena and the DAM's
+        batch-norm moving statistics, never the critics --, updated after every G step, checkpointed, monitored and written as
+        averaged-weights checkpoints; None: no average"""
         self.net = net
         self.batch_size = batch_size
         self.num_cls = num_cls
@@ -341,6 +345,8 @@ class Trainer(object):
         # schedule's later `dis_sub_iter += dis_sub_iter_inc` (a local of train(), :829/:886) never reaches them
         self._obj_dis_sub_iter, self._obj_gen_sub_iter = self.dis_sub_iter, self.gen_sub_iter
         self._build_optimizers()
+        self.ema = None if ema_decay is None else EMA(
+            self.g_arena, [v for v in net.adapt_vars if v.pnp_kind == "bn_moving"], ema_decay)
 
     def _build_optimizers(self):
         """adversarial.py:633-656"""
@@ -440,6 +446,8 @@ class Trainer(object):
     def g_apply(self):
         scale = self.dp.finish_backward(self.g_arena)
         self.gen_optimizer.step(grad_scale=scale)
+        if self.ema is not None:
+            self.ema.update()
         self.global_step += 1
 
     def evaluate(self, ct_batch, ct_labels_onehot):
@@ -450,6 +458,20 @@ class Trainer(object):
             dice, arr = self.net.dice_eval(out["logits"], ct_labels_onehot)
             cm = F.confusion_counts(out["logits"], ct_labels_onehot)
         return {"dice_eval": float(dice), "dice_arr": [float(a) for a in arr], "confusion_matrix": cm.cpu().numpy()}
+
+    EMA_TAGS = ("ema_ct_dice_eval_c1_lv_myo", "ema_ct_dice_eval_c2_la_blood", "ema_ct_dice_eval_c3_lv_blood", "ema_ct_dice_eval_c4_aa")
+
+    def ema_stats(self, step, ct_batch, ct_batch_y, log_dir=None):
+        """evaluate's CT forward and per-organ Dice with the averaged weights swapped in (no critic runs: their batch-statistics
+        BN would move) -> the EMA_TAGS scalars, written to `log_dir`'s event file with `step` after the pass's own summaries"""
+        if ct_batch_y.dim() == 3:
+            ct_batch_y = F.one_hot(ct_batch_y, self.num_cls or self.net.n_class)
+        with self.ema.swapped(), torch.no_grad():
+            logits = self.net.segment(ct_batch, "ct", 1.0, front_bn=False, joint_bn=False)["logits"]
+            _, arr = self.net.dice_eval(logits, ct_batch_y)
+            scalars = dict(zip(self.EMA_TAGS, [float(arr[i]) for i in range(1, 5)]))
+        summary.write_pass(self, log_dir, step, scalars)
+        return scalars
 
     # the reference's TensorBoard scalar tags (adversarial.py:664-683), written as JSON lines because TensorBoard is not a dependency
     SCALAR_TAGS = ("fixed_coeff_reg", "discriminator_loss", "generator_loss", "ct_dice_eval_c1_lv_myo", "ct_dice_eval_c2_la_blood",
@@ -616,6 +638,9 @@ class Trainer(object):
         st.update(self.gen_optimizer.slot_state())
         st["pnp/learning_rate"] = np.float32(self.dis_optimizer.get_lr())       # TF names these two scalars 'Variable_k' by
         st["pnp/global_step"] = np.int64(self.global_step)                      # creation order; stable keys here
+        if self.ema is not None:
+            self.ema.average_over_ranks(self.dp)
+            st.update(self.ema.state())
         return st
 
     def load_optimizer_state(self, d, clear_rms=False):
@@ -648,6 +673,7 @@ class Trainer(object):
             return save_path
         os.makedirs(output_path, exist_ok=True)
         cfg = self.train_config
+        resumed = {}
         if restore and restored_path and os.path.exists(os.path.join(restored_path, "latest.npz")):
             ck = os.path.join(restored_path, "latest.npz")
             self.net.restore(ck, no_gan=cfg.get("restore_from_baseline", False), clear_rms=cfg.get("clear_rms", False))
@@ -657,6 +683,7 @@ class Trainer(object):
                 self.net.adapt_copy_weights()
             else:
                 self.load_optimizer_state(self.net.last_restored, clear_rms=cfg.get("clear_rms", False))
+                resumed = self.net.last_restored
         # data parallel: every replica continues from rank 0's variables (weights, frozen parts, BN statistics, slots)
         self.dp.broadcast_variables(rt.global_variables())
         for opt_ in (self.dis_optimizer, self.gen_optimizer):
@@ -665,6 +692,8 @@ class Trainer(object):
         if self.lr_update_flag:
             self.dis_optimizer.set_lr(self.LR_refresh)
             self.gen_optimizer.set_lr(self.LR_refresh)
+        if self.ema is not None and not self.ema.load_state(resumed):     # a resumed average continues; otherwise it starts here
+            self.ema.init_from_live()
         B, r, nc = self.batch_size, self.dp.rank, self.num_cls or 5
         mr_src = pick_source(self.mr_source, self.mr_train_list, B, 1234 + r, nc)
         ct_src = pick_source(self.ct_source, self.ct_train_list, B, 4321 + r, nc, shift=0.3, scale=0.8)
@@ -699,8 +728,11 @@ class Trainer(object):
                     tag = str(self.train_config.get("tag", ""))      # FileWriter(output_path + "/train_log" + tag) (adversarial.py:807-808)
                     for sub, detail, cs, ms in (("train_log", False, ct_src, mr_src), ("val_log", True, ct_val, mr_val)):
                         (ct, cty), (mr, mry) = cs.next(), ms.next()
-                        self.output_minibatch_stats(step, to_device(ct, dev), to_device(cty, dev), to_device(mr, dev), to_device(mry, dev),
+                        ct, cty = to_device(ct, dev), to_device(cty, dev)
+                        self.output_minibatch_stats(step, ct, cty, to_device(mr, dev), to_device(mry, dev),
                                                     os.path.join(output_path, sub + tag), detail, **img)
+                        if detail and self.ema is not None:
+                            self.ema_stats(step, ct, cty, os.path.join(output_path, sub + tag))
                 if step % ckpt_space == 0 and step != 0:
                     self.save(save_path, output_path)
                     # "Model has been restored for re-allocation" (adversarial.py:929-935): the reference re-reads the checkpoint it

@@ -1,6 +1,6 @@
 // HBM-bound kernels of the PnP-AdaNet hot path for sm_90a: batch-norm statistics / apply / backward,
 // activation + residual skip, dropout, 2x2 max-pool, mirror pad, phase shift (pixel shuffle) and the
-// discriminator-input gather, per-pixel softmax losses, FC + WGAN means, L2 sums, fused Adam / RMSProp+clip.
+// discriminator-input gather, per-pixel softmax losses, FC + WGAN means, L2 sums, fused Adam / RMSProp+clip, the weights' moving average.
 // All are coalesced 128-bit streaming kernels with warp-shuffle / shared-memory reductions and double
 // precision global accumulators; grids are sized in multiples of the 132 SMs.
 #include "common.cuh"
@@ -1143,6 +1143,55 @@ __global__ void __launch_bounds__(256) fill_kernel(float* __restrict__ p, float 
   if (blockIdx.x == 0 && threadIdx.x < (n & 3)) p[(n4 << 2) + threadIdx.x] = v;
 }
 
+// tf.train.ExponentialMovingAverage(decay, num_updates=n): c = 1 - min(decay, (1 + n) / (10 + n)), every operation rounded on its own
+__global__ void ema_advance_kernel(long long* num_updates, float decay, float* c) {
+  pnp_pdl_enter();
+  const long long n = *num_updates;
+  const float nf = __ll2float_rn(n);
+  const float d = fminf(decay, __fdiv_rn(__fadd_rn(1.f, nf), __fadd_rn(10.f, nf)));
+  *c = __fsub_rn(1.f, d);
+  *num_updates = n + 1;
+}
+
+__device__ __forceinline__ float ema1(float s, float x, float c) { return __fsub_rn(s, __fmul_rn(__fsub_rn(s, x), c)); }
+
+// one CTA per 1024-float chunk of the shadow: chunks below arena_chunks mirror the live arena (float4), the rest follow the table
+template <bool SWAP>
+__global__ void __launch_bounds__(256)
+ema_kernel(float* __restrict__ shadow, float* __restrict__ arena, long long arena_chunks, const pnp_ema_chunk* __restrict__ table,
+           const float* __restrict__ c_ptr) {
+  pnp_pdl_enter();
+  const long long b = blockIdx.x;
+  float* s = shadow + b * 1024;
+  if (b < arena_chunks) {
+    float4* x4 = reinterpret_cast<float4*>(arena + b * 1024) + threadIdx.x;
+    float4* s4 = reinterpret_cast<float4*>(s) + threadIdx.x;
+    const float4 x = *x4;
+    float4 v = *s4;
+    if (SWAP) {
+      *x4 = v;
+      *s4 = x;
+    } else {
+      const float c = *c_ptr;
+      v.x = ema1(v.x, x.x, c); v.y = ema1(v.y, x.y, c); v.z = ema1(v.z, x.z, c); v.w = ema1(v.w, x.w, c);
+      *s4 = v;
+    }
+    return;
+  }
+  const pnp_ema_chunk e = table[b - arena_chunks];
+  const float c = SWAP ? 0.f : *c_ptr;
+  const int len = (int)min(e.len, 1024LL);
+  for (int i = threadIdx.x; i < len; i += 256) {
+    const float x = e.live[i];
+    if (SWAP) {
+      e.live[i] = s[i];
+      s[i] = x;
+    } else {
+      s[i] = ema1(s[i], x, c);
+    }
+  }
+}
+
 }  // namespace
 
 #define S_ ((cudaStream_t)stream)
@@ -1583,6 +1632,37 @@ extern "C" int pnp_momentum_step(float* theta, const float* grad, float* accum, 
 extern "C" int pnp_fill(float* p, float v, long long n, void* stream) {
   if (!p || n <= 0) return PNP_ERR_BAD_ARG;
   pnp_launch(fill_kernel, grid_for(n / 4 + 1, 256 * 4), 256, 0, S_, p, v, n);
+  PNP_LAUNCH_CHECK();
+  return PNP_OK;
+}
+
+// shadow = arena_n + 1024 * table_n floats; the grid is one CTA per chunk
+static int ema_check(const float* shadow, const float* arena, long long arena_n, const pnp_ema_chunk* table, int table_n) {
+  if (!shadow || !arena || arena_n <= 0 || (arena_n % 1024) != 0 || table_n < 0 || (table_n > 0 && !table)) return PNP_ERR_BAD_ARG;
+  if (arena_n / 1024 + table_n > 0x7FFFFFFFLL) return PNP_ERR_BAD_ARG;
+  return PNP_OK;
+}
+
+extern "C" int pnp_ema_advance(long long* num_updates, float decay, float* c, void* stream) {
+  if (!num_updates || !c || !(decay > 0.f && decay < 1.f)) return PNP_ERR_BAD_ARG;
+  pnp_launch(ema_advance_kernel, 1, 1, 0, S_, num_updates, decay, c);
+  PNP_LAUNCH_CHECK();
+  return PNP_OK;
+}
+
+extern "C" int pnp_ema_update(float* shadow, const float* arena, long long arena_n, const pnp_ema_chunk* table, int table_n, const float* c,
+                              void* stream) {
+  if (ema_check(shadow, arena, arena_n, table, table_n) || !c) return PNP_ERR_BAD_ARG;
+  pnp_launch(ema_kernel<false>, (unsigned)(arena_n / 1024 + table_n), 256, 0, S_, shadow, const_cast<float*>(arena), arena_n / 1024,
+             table, c);
+  PNP_LAUNCH_CHECK();
+  return PNP_OK;
+}
+
+extern "C" int pnp_ema_swap(float* shadow, float* arena, long long arena_n, const pnp_ema_chunk* table, int table_n, void* stream) {
+  if (ema_check(shadow, arena, arena_n, table, table_n)) return PNP_ERR_BAD_ARG;
+  pnp_launch(ema_kernel<true>, (unsigned)(arena_n / 1024 + table_n), 256, 0, S_, shadow, arena, arena_n / 1024, table,
+             (const float*)nullptr);
   PNP_LAUNCH_CHECK();
   return PNP_OK;
 }

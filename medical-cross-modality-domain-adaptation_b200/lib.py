@@ -122,10 +122,18 @@ def _save(state, model_path, global_step=None):
 
 def save_checkpoint(trainer, save_path, output_path):
     """both trainers' save: trainer.checkpoint_state() as <save_path>-<global_step>.npz and <output_path>/latest.npz, written by
-    rank 0 while every rank waits"""
+    rank 0 while every rank waits.  A trainer with a weights' moving average (trainer.ema) also gets the averaged-weights
+    checkpoints <save_path>-<global_step>_ema.npz and <output_path>/latest_ema.npz (ema.averaged_weights), which every
+    consumer of a checkpoint reads as it reads the others"""
+    from . import runtime as rt
+    from .ema import averaged_weights
     st = trainer.checkpoint_state()
+    avg = averaged_weights(st, rt.graph.order) if getattr(trainer, "ema", None) is not None else None
 
     def write():
         _save(st, save_path, global_step=trainer.global_step)
         _save(st, os.path.join(output_path, "latest"))
+        if avg is not None:
+            _save(avg, "%s-%d_ema" % (save_path, int(trainer.global_step)))
+            _save(avg, os.path.join(output_path, "latest_ema"))
     trainer.dp.save_checkpoint(write)

@@ -22,6 +22,7 @@ from . import optim
 from . import parallel
 from . import summary
 from .data import pick_source, to_device
+from .ema import EMA
 from .lib import _label_decomp, save_checkpoint
 from .networks import FRONT, BACK, SegmenterHalf, SegmenterTail
 
@@ -143,7 +144,10 @@ class Trainer(object):
 
     def __init__(self, net, train_list, val_list, num_cls, batch_size, test_nii_list=None, test_label_list=None,
                  optimizer="momentum", opt_kwargs={}, num_epochs=100, checkpoint_space=500, lr_update_flag=False, source=None,
-                 val_source=None):
+                 val_source=None, ema_decay=None):
+        """`ema_decay`: keep an exponential moving average (ema.EMA) of the optimizer's variables and of every batch-norm moving
+        statistic, updated after every optimizer step, checkpointed, monitored and written as averaged-weights checkpoints;
+        None: no average"""
         self.net = net
         self.batch_size = batch_size
         self.num_cls = num_cls
@@ -160,6 +164,8 @@ class Trainer(object):
         self.dp = parallel.DataParallel()
         self._graph = None           # the captured train step (runtime.StepGraph), None: eager
         self._build_optimizer()
+        self.ema = None if ema_decay is None else EMA(
+            self.arena, [v for v in rt.global_variables() if v.pnp_kind == "bn_moving"], ema_decay)
 
     def _build_optimizer(self):
         """source_segmenter.py:357-381: Adam over every trainable variable, loss = cost + regularizer"""
@@ -192,6 +198,8 @@ class Trainer(object):
         torch.autograd.backward([wce, dice], [self._g_cross, self._g_dice])
         scale = self.dp.finish_backward(self.arena)
         self.optimizer.step(grad_scale=scale)
+        if self.ema is not None:
+            self.ema.update()
         self.global_step += 1
         return wce, dice
 
@@ -262,6 +270,7 @@ class Trainer(object):
         if epochs == 0:
             return save_path
         os.makedirs(output_path, exist_ok=True)
+        d = {}
         if restore and restored_path and os.path.exists(os.path.join(restored_path, "latest.npz")):
             self.net.restore(os.path.join(restored_path, "latest.npz"))
             # tf.train.Saver() also brings back the Adam slots, the learning-rate variable and global_step (:398,:446-452)
@@ -282,6 +291,8 @@ class Trainer(object):
         else:
             self.dp.broadcast_params(self.optimizer.m)
             self.dp.broadcast_params(self.optimizer.v)
+        if self.ema is not None and not self.ema.load_state(d):     # a resumed average continues; otherwise it starts here
+            self.ema.init_from_live()
         src = pick_source(self.source, self.train_list, self.batch_size, 1234 + self.dp.rank, self.num_cls)
         # the validation queue of source_segmenter.py:325,467 (val_list), else a second synthetic stream
         val_src = pick_source(self.val_source, self.val_list, self.batch_size, 4321 + self.dp.rank, self.num_cls)
@@ -299,6 +310,8 @@ class Trainer(object):
                     # source_segmenter.py:498-505: a validation batch right after it, always with the per-organ table
                     vx, vy = self.feed(*val_src.next())
                     self.val_stats(vx, vy, step, os.path.join(output_path, "val_log"), detail=True, **img)
+                    if self.ema is not None:
+                        self.ema_val_stats(vx, vy, step, os.path.join(output_path, "val_log"))
                 if step % self.checkpoint_space == 0 and step > 10000:
                     self.save(save_path, output_path)
                     self.optimizer.set_lr(self.optimizer.get_lr() * 0.9)
@@ -310,6 +323,9 @@ class Trainer(object):
         st.update(self.optimizer.slot_state())
         st["pnp/learning_rate"] = np.float32(self.optimizer.get_lr())
         st["pnp/global_step"] = np.int64(self.global_step)
+        if self.ema is not None:
+            self.ema.average_over_ranks(self.dp)
+            st.update(self.ema.state())
         return st
 
     def save(self, save_path, output_path):
@@ -328,6 +344,18 @@ class Trainer(object):
                 _indicator_eval(self.net.confusion_matrix(logits, batch_y).cpu().numpy())
             self._summaries(log_dir, step, self.VAL_IMAGE_TAGS, image_summaries, logits, batch_x, batch_y, wce, dice)
         return {"loss": self.net.cost_value(wce, dice), "dice_eval": float(d), "dice_arr": [float(a) for a in arr]}
+
+    EMA_TAGS = ("ema_dice_eval", "ema_dice_eval_c1", "ema_dice_eval_c2", "ema_dice_eval_c3", "ema_dice_eval_c4")
+
+    def ema_val_stats(self, batch_x, batch_y, step=None, log_dir=None):
+        """val_stats' forward and Dice with the averaged weights swapped in (nothing else runs under the swap) -> the EMA_TAGS
+        scalars, written to `log_dir`'s event file with `step` after the pass's own summaries"""
+        with self.ema.swapped(), torch.no_grad():
+            logits = self.net.forward(batch_x, keep_prob=1.0, main_bn=False, adapt_bn=False)
+            d, arr = self.net.dice_eval(logits, batch_y)
+            scalars = dict(zip(self.EMA_TAGS, [float(d)] + [float(arr[i]) for i in range(1, 5)]))
+        summary.write_pass(self, log_dir, step, scalars)
+        return scalars
 
     # ---- test protocol on NIfTI subjects (source_segmenter.py:572-675) -----------------------------------------------
     def _logits(self, x):

@@ -72,9 +72,17 @@ def main(phase, argv=None):
                     help="with --volumes: add a smooth bias field, a contrast and an offset to the MR and CT training slices")
     ap.add_argument("--image-summaries", action="store_true",
                     help="also write the reference's TensorBoard image summaries (prediction, input slice, ground truth) every display step")
+    ap.add_argument("--ema-decay", type=float, default=None, metavar="D",
+                    help="keep an exponential moving average of the trained weights with this decay (0 < D < 1): checkpointed, "
+                         "monitored as ema_* scalars and written as averaged-weights checkpoints *_ema.npz")
     a = ap.parse_args(argv)
     if (a.elastic or a.intensity) and not a.volumes:
         ap.error("--elastic / --intensity augment the slices drawn with --volumes; give --volumes")
+    if a.ema_decay is not None:
+        if a.phase == "pre-train":
+            ap.error("--ema-decay averages the generator's weights; the pre-train phase runs no generator step")
+        if not 0.0 < a.ema_decay < 1.0:
+            ap.error("--ema-decay must lie in (0, 1)")
     logging.basicConfig(level=logging.INFO)
     parallel.init_from_env()
     if a.conv_backend:
@@ -100,7 +108,7 @@ def main(phase, argv=None):
                                     ("mr_val_source", "mr_val_volumes", 2234, {}), ("ct_val_source", "ct_val_volumes", 5321, {})):
             sources[key] = volume_source(os.path.join(a.lists, name), a.batch_size, seed + rank, **kw)
     trainer = drn.Trainer(net, mr_train, mr_val, ct_train, ct_val, num_cls=num_cls, batch_size=a.batch_size,
-                          opt_kwargs=dict(opt_kwargs), train_config=tc, **sources)
+                          opt_kwargs=dict(opt_kwargs), train_config=tc, ema_decay=a.ema_decay, **sources)
     print("Now start training...")
     return trainer.train(output_path=out, restored_path=out, training_iters=a.training_iters or tc["training_iters"],
                          epochs=a.epochs or tc["epochs"], dropout=a.keep_prob, image_summaries=a.image_summaries)

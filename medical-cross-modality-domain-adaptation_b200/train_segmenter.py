@@ -72,9 +72,14 @@ def main(argv=None):
                     help="with --train-volumes: add a smooth bias field, a contrast and an offset to the training slices")
     ap.add_argument("--image-summaries", action="store_true",
                     help="also write the reference's TensorBoard image summaries (prediction, input slice, ground truth) every display step")
+    ap.add_argument("--ema-decay", type=float, default=None, metavar="D",
+                    help="keep an exponential moving average of the trained weights with this decay (0 < D < 1): checkpointed, "
+                         "monitored as ema_* scalars and written as averaged-weights checkpoints *_ema.npz")
     a = ap.parse_args(argv)
     if (a.elastic or a.intensity) and not a.train_volumes:
         ap.error("--elastic / --intensity augment the slices drawn from --train-volumes; give --train-volumes")
+    if a.ema_decay is not None and not 0.0 < a.ema_decay < 1.0:
+        ap.error("--ema-decay must lie in (0, 1)")
     logging.basicConfig(level=logging.INFO)
     parallel.init_from_env()
     if a.conv_backend:
@@ -89,7 +94,8 @@ def main(argv=None):
                (("source", a.train_volumes, 1234, {"elastic": a.elastic, "intensity": a.intensity}),
                 ("val_source", a.val_volumes, 4321, {})) if path}
     trainer = drn.Trainer(net, train_list=train_list, val_list=val_list, num_cls=num_cls, batch_size=a.batch_size, opt_kwargs=dict(opt_kwargs),
-                          checkpoint_space=checkpoint_space, optimizer=optimizer, lr_update_flag=False, **sources)
+                          checkpoint_space=checkpoint_space, optimizer=optimizer, lr_update_flag=False, ema_decay=a.ema_decay,
+                          **sources)
     print("Now start training...")
     return trainer.train(output_path=a.output_path, restored_path=a.output_path, training_iters=a.training_iters,
                          epochs=a.epochs, restore=restore, dropout=a.keep_prob, image_summaries=a.image_summaries)
