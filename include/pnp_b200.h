@@ -313,6 +313,34 @@ int pnp_ema_update(float* shadow, const float* arena, long long arena_n, const p
                    void* stream);
 int pnp_ema_swap(float* shadow, float* arena, long long arena_n, const pnp_ema_chunk* table, int table_n, void* stream);
 
+/* ---- batch-norm population statistics (PreciseBN / AdaBN re-estimation) ------------------------------------------------------
+ * Over N batch-statistics forward passes, layer l's fp64 per-channel sums S1_b = sum z, S2_b = sum z^2 (what pnp_bn_stats or the
+ * fused convolution epilogue writes) are added up, and the moving statistics are replaced by the pooled statistics of every
+ * value seen.  Every operation is fp64 and rounded on its own (no FMA contraction):
+ *   pnp_bn_accumulate: acc[c] += sum[c]; acc[C + c] += sumsq[c] for every entry and channel c < C (one launch per pass, so the
+ *                      passes are added in the order they ran).
+ *   pnp_bn_population: m = acc[c] / n; v = acc[C + c] / n - m * m; v = 0 if v < 0 (a NaN passes); moving_mean[c] = (float)m;
+ *                      moving_var[c] = (float)(n > 1 ? v * (n / (n - 1)) : v), with n = count = sum of the passes' B * Ho * Wo.
+ * `table` is HOST memory of n >= 1 entries; its contents travel in the launch's parameters (64 entries per launch), so the
+ * caller may reuse it once the call returns, and a captured graph keeps the pointers it was captured with.  The buffers the
+ * entries point to are device memory; acc is [2C] fp64.  Null table or pointers, n < 1, C < 1 or C > 1024, count < 1:
+ * PNP_ERR_BAD_ARG, and nothing is launched. */
+typedef struct {
+  const double* sum;
+  const double* sumsq;
+  double* acc;
+  int C;
+} pnp_bn_acc_entry;
+typedef struct {
+  const double* acc;
+  long long count;
+  float* moving_mean;
+  float* moving_var;
+  int C;
+} pnp_bn_pop_entry;
+int pnp_bn_accumulate(const pnp_bn_acc_entry* table, int n, void* stream);
+int pnp_bn_population(const pnp_bn_pop_entry* table, int n, void* stream);
+
 /* ---- evaluation: 3-D surface distances ---------------------------------------------------------------------------------------
  * Per-class surface distances between a predicted label volume P and a ground truth G (medpy.metric.binary.assd / hd as the
  * papers' evaluation calls them).  pred and gt are uint8 [n0][n1][n2] (n2 fastest) on the device; labels >= C count as

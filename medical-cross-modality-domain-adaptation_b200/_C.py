@@ -27,6 +27,16 @@ class TcEpilogue(ctypes.Structure):
                 ("y_hi", c_void_p), ("y_lo", c_void_p)]
 
 
+class BnAccEntry(ctypes.Structure):
+    """pnp_bn_acc_entry"""
+    _fields_ = [("sum", c_void_p), ("sumsq", c_void_p), ("acc", c_void_p), ("C", c_int)]
+
+
+class BnPopEntry(ctypes.Structure):
+    """pnp_bn_pop_entry"""
+    _fields_ = [("acc", c_void_p), ("count", c_ll), ("moving_mean", c_void_p), ("moving_var", c_void_p), ("C", c_int)]
+
+
 def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
@@ -104,6 +114,8 @@ SIGNATURES = {
     "pnp_ema_advance": [P, c_float, P, P],
     "pnp_ema_update": [P, P, c_ll, P, c_int, P, P],
     "pnp_ema_swap": [P, P, c_ll, P, c_int, P],
+    "pnp_bn_accumulate": [ctypes.POINTER(BnAccEntry), c_int, P],
+    "pnp_bn_population": [ctypes.POINTER(BnPopEntry), c_int, P],
     "pnp_surface_distance_workspace": [c_int, c_int, c_int, c_int, P],
     "pnp_surface_distance": [P, P, c_int, c_int, c_int, c_int, P, P, c_ll, P, P],
     "pnp_surface_distance_pct_workspace": [c_int, c_int, c_int, c_int, P],

@@ -619,6 +619,23 @@ class Trainer(object):
     def release_graphs(self):
         self._graph = self._d_graph = self._g_graph = None
 
+    def recalibrate_bn(self, ct_source, batches, scope="dam"):
+        """re-estimate batch-norm moving statistics as exact population statistics (bnstats.py; DESIGN 6.1) over `batches`
+        forwards of the CT stream on images from `ct_source` (.next() -> (images, labels), labels ignored; the network's batch
+        size): keep_prob 1, batch-statistics batch norm on the covered layers, every other layer as at inference.  On CT
+        slices this is AdaBN.  scope 'dam': the 20 adapt_* batch norms.  'all': also the 10 of the shared groups 7-9 -- the
+        result is then a CT-inference model, and the MR stream, which shares those groups, no longer normalises them with
+        the source segmenter's statistics.  The critics never run.  Captured steps are released.  -> (covered variable names,
+        slice count).  ValueError: batches < 1 or a wrong batch size; NotImplementedError under data parallelism."""
+        from . import bnstats
+        if scope not in ("dam", "all"):
+            raise ValueError("scope must be 'dam' or 'all', got %r" % (scope,))
+        shared = ("group_7", "group_8", "group_9") if scope == "all" else ()
+        covered = [v for v in rt.global_variables() if v.pnp_kind == "bn_moving"
+                   and (v.pnp_name.startswith("adapt_") or v.pnp_name.split("/")[0] in shared)]
+        fwd = lambda x: self.net.segment(x, "ct", 1.0, front_bn=True, joint_bn=(scope == "all"))
+        return bnstats.recalibrate(self, ct_source, batches, bnstats.covered_statistics(covered), fwd)
+
     def joint_step(self, mr_batch, ct_batch, keep_prob=0.75, ct_batch_g=None):
         """one full adversarial step (D update + clip, then G update); replays the captured graph when there is one.
         `ct_batch_g`: the fresh CT batch the reference dequeues for the generator update (adversarial.py:869-873);

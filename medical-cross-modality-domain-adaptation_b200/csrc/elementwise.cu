@@ -191,6 +191,35 @@ __global__ void bn_finalize_kernel(const double* __restrict__ sum, const double*
   invstd[c] = is;
 }
 
+// population statistics of many batch-statistics passes: one thread per (entry, channel).  The entries travel by value in the
+// kernel parameters (kBnTable per launch, 2.0 / 2.5 KB of the 4 KB parameter space); the grid's y is the entry, its x covers
+// up to 1024 channels.  acc = [A1[C] | A2[C]], summed in pass order, every operation rounded on its own
+constexpr int kBnTable = 64;
+struct BnAccTable { pnp_bn_acc_entry e[kBnTable]; };
+struct BnPopTable { pnp_bn_pop_entry e[kBnTable]; };
+
+__global__ void __launch_bounds__(256) bn_accumulate_kernel(const __grid_constant__ BnAccTable t) {
+  pnp_pdl_enter();
+  const pnp_bn_acc_entry& e = t.e[blockIdx.y];
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= e.C) return;
+  e.acc[c] = __dadd_rn(e.acc[c], e.sum[c]);
+  e.acc[e.C + c] = __dadd_rn(e.acc[e.C + c], e.sumsq[c]);
+}
+
+__global__ void __launch_bounds__(256) bn_population_kernel(const __grid_constant__ BnPopTable t) {
+  pnp_pdl_enter();
+  const pnp_bn_pop_entry& e = t.e[blockIdx.y];
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= e.C) return;
+  const double n = (double)e.count;
+  const double m = __ddiv_rn(e.acc[c], n);
+  double v = __dsub_rn(__ddiv_rn(e.acc[e.C + c], n), __dmul_rn(m, m));
+  if (v < 0.0) v = 0.0;             // a NaN passes through
+  e.moving_mean[c] = (float)m;
+  e.moving_var[c] = (float)(e.count > 1 ? __dmul_rn(v, __ddiv_rn(n, (double)(e.count - 1))) : v);
+}
+
 __global__ void __launch_bounds__(256)
 bn_act_apply_kernel(const float* __restrict__ z, const float* __restrict__ scale, const float* __restrict__ shift,
                     const float* __restrict__ skip, int Cs, int skip_off, int act, float* __restrict__ y,
@@ -1214,6 +1243,37 @@ extern "C" int pnp_bn_finalize(const double* sum, const double* sumsq, long long
   pnp_launch(bn_finalize_kernel, pnp_cdiv(C, 128), 128, 0, S_, sum, sumsq, M, C, gamma, beta, moving_mean, moving_var, training, scale,
                                                        shift, mean, invstd);
   PNP_LAUNCH_CHECK();
+  return PNP_OK;
+}
+
+extern "C" int pnp_bn_accumulate(const pnp_bn_acc_entry* table, int n, void* stream) {
+  if (!table || n < 1) return PNP_ERR_BAD_ARG;
+  for (int i = 0; i < n; ++i)
+    if (!table[i].sum || !table[i].sumsq || !table[i].acc || table[i].C < 1 || table[i].C > 1024) return PNP_ERR_BAD_ARG;
+  for (int i = 0; i < n; i += kBnTable) {
+    const int k = min(kBnTable, n - i);
+    BnAccTable t = {};
+    int cmax = 1;
+    for (int j = 0; j < k; ++j) { t.e[j] = table[i + j]; cmax = max(cmax, t.e[j].C); }
+    pnp_launch(bn_accumulate_kernel, dim3(pnp_cdiv(cmax, 256), k), 256, 0, S_, t);
+    PNP_LAUNCH_CHECK();
+  }
+  return PNP_OK;
+}
+
+extern "C" int pnp_bn_population(const pnp_bn_pop_entry* table, int n, void* stream) {
+  if (!table || n < 1) return PNP_ERR_BAD_ARG;
+  for (int i = 0; i < n; ++i)
+    if (!table[i].acc || !table[i].moving_mean || !table[i].moving_var || table[i].C < 1 || table[i].C > 1024 || table[i].count < 1)
+      return PNP_ERR_BAD_ARG;
+  for (int i = 0; i < n; i += kBnTable) {
+    const int k = min(kBnTable, n - i);
+    BnPopTable t = {};
+    int cmax = 1;
+    for (int j = 0; j < k; ++j) { t.e[j] = table[i + j]; cmax = max(cmax, t.e[j].C); }
+    pnp_launch(bn_population_kernel, dim3(pnp_cdiv(cmax, 256), k), 256, 0, S_, t);
+    PNP_LAUNCH_CHECK();
+  }
   return PNP_OK;
 }
 

@@ -393,6 +393,9 @@ def _geometry(x_shape, w_shape, cfg):
 # fold inference-mode batch norm + skip + activation into the wgmma epilogue (PNP_FUSE_EPILOGUE=0: separate apply kernel)
 FUSE_EPILOGUE = os.environ.get("PNP_FUSE_EPILOGUE", "1") != "0"
 
+# the active bnstats.Collector while batch-norm statistics are re-estimated (bnstats.collecting), else None
+BN_COLLECTOR = None
+
 
 def layer_forward(x, W, cfg, skip=None, save=True, planes_only=False):
     """returns (y, saved) -- `saved` is None when save is False (inference / frozen sub-graph).
@@ -444,6 +447,8 @@ def layer_forward(x, W, cfg, skip=None, save=True, planes_only=False):
     if bn is not None:
         if cfg.bn_training and not stats_done:
             call("pnp_bn_stats", ptr(z), M, C, ptr(stats[0]), ptr(stats[1]), rt.stream())
+        if cfg.bn_training and BN_COLLECTOR is not None:
+            BN_COLLECTOR.add(bn, stats, M)
         vec = torch.empty(2, C, dtype=torch.float32, device=dev)
         mean, invstd = vec[0], vec[1]
         if cfg.bn_training:

@@ -149,6 +149,9 @@ class _BNOnly(torch.autograd.Function):
         C = x.shape[-1]
         M = x.numel() // C
         dev = x.device
+        if training and F.BN_COLLECTOR is not None:
+            raise RuntimeError("batch-norm recalibration covers the convolution layers' batch norms only; %s is a standalone one"
+                               % bn.moving_mean.pnp_name)
         stats = F._zeros_f64(2 * C, dev) if training else None
         if training:
             call("pnp_bn_stats", ptr(x), M, C, ptr(stats[:C]), ptr(stats[C:]), rt.stream())

@@ -211,6 +211,19 @@ class Trainer(object):
                                       keep_prob, warmup, self.trainables, (self.arena,), detach=True)
         return self._graph is not None
 
+    def release_graphs(self):
+        self._graph = None
+
+    def recalibrate_bn(self, source, batches):
+        """re-estimate every batch norm's moving statistics (all 30) as exact population statistics (bnstats.py; DESIGN 6.1)
+        over `batches` forwards on images from `source` (.next() -> (images, labels), labels ignored; the network's batch
+        size): keep_prob 1, batch-statistics batch norm.  Captured steps are released.  -> (covered variable names, slice
+        count).  ValueError: batches < 1 or a wrong batch size; NotImplementedError under data parallelism."""
+        from . import bnstats
+        covered = bnstats.covered_statistics([v for v in rt.global_variables() if v.pnp_kind == "bn_moving"])
+        fwd = lambda x: self.net.forward(x, 1.0, main_bn=True, adapt_bn=True)
+        return bnstats.recalibrate(self, source, batches, covered, fwd)
+
     def train_step_replay(self, batch_x, batch_y, keep_prob=0.75):
         if not rt.StepGraph.fits(self._graph, keep_prob):
             return self.train_step(batch_x, batch_y, keep_prob)
