@@ -3,7 +3,8 @@ that medpy.metric.binary.hd95 computes, HD_q = np.percentile(np.hstack((da, db))
 db = d(v, dA) over v in dB, the border sets and distances of oracle/surface_exact.py.
 
 * `scipy_distances` / `brute_distances` give the per-class arrays (da, db) of surface_exact's two forms -- the values its
-  `scipy_raw` / `brute_raw` sum and maximise: scipy.ndimage's distance transform, and an all-pairs search for small volumes;
+  `scipy_raw` / `brute_raw` sum and maximise: scipy.ndimage's distance transform, and an all-pairs search for small volumes
+  (oracle/surface_kdtree.py's `kdtree_distances`, a nearest-neighbour search fast at native CT size, is the third form);
 * `hd_percentile` is medpy's line on them;
 * `percentile_linear` restates numpy's default `linear` percentile operation by operation (the formula the kernel implements);
   the CPU tests hold it equal to np.percentile.
@@ -16,6 +17,7 @@ import numpy as np
 from scipy import ndimage
 
 from oracle import surface_exact as se
+from oracle import surface_kdtree as sk
 
 
 def scipy_distances(pred, gt, num_cls, spacing=None):
@@ -46,8 +48,10 @@ def brute_distances(pred, gt, num_cls, spacing=None):
 
 def hd_percentile(pred, gt, num_cls, q, spacing=None, form="scipy"):
     """[num_cls]: medpy.metric.binary.hd95's pooled percentile, np.percentile(np.hstack((da, db)), q), per class (index 0 and
-    classes with an empty border: NaN); `form` "scipy" or "brute" picks the distance arrays"""
-    dist = (scipy_distances if form == "scipy" else brute_distances)(pred, gt, num_cls, spacing)[0]
+    classes with an empty border: NaN); `form` "scipy", "brute" or "kdtree" (oracle/surface_kdtree.py) picks the distance
+    arrays"""
+    forms = {"scipy": scipy_distances, "brute": brute_distances, "kdtree": sk.kdtree_distances}
+    dist = forms[form](pred, gt, num_cls, spacing)[0]
     out = np.full(num_cls, math.nan)
     for c in range(1, num_cls):
         da, db = dist[c]
