@@ -471,6 +471,29 @@ int pnp_native_labels(const float* scores, int n0, int n1, int n2, int C, const 
 int pnp_native_labels_ensemble(const float* scores, int K, int n0, int n1, int n2, int C, const float* maps, int m0, int m1, int m2,
                                uint8_t* out, const uint8_t* gt, long long* cm, void* stream);
 
+/* ---- native-grid labels of any number of predictions, one launch per prediction (resample.cu) ------------------------------
+ * The streaming form of pnp_native_labels_ensemble, without its member cap and without K resident score volumes (the heart
+ * localisation's sliding windows, native.py / localise.py).  sums: fp32 C-order [m0][m1][m2][C] and covered: uint8 [m0][m1][m2],
+ * both on the device and zeroed by the caller once before the first prediction (offsets into sums are 64-bit: m0*m1*m2*C may reach
+ * 2^31 and beyond).
+ * pnp_native_accumulate samples one prediction (scores [n0][n1][n2][C], map: as pnp_native_labels takes them) at every native
+ *   voxel with pnp_native_labels' coordinate, coverage, taps and lerps (one shared kernel body).  Where the prediction covers the
+ *   voxel: if covered is 0 its class scores are stored as they are and covered is set to 1, otherwise they are added to sums (fp32,
+ *   each sum rounded).  Voxels it does not cover are not touched.
+ * pnp_native_accumulated_labels: out (uint8) is the first maximum over c of sums (the lowest index wins a tie) where covered is
+ *   non-zero and 0 elsewhere; cm (optional with gt) as pnp_native_labels counts it (the call zeroes cm first).
+ * K accumulate launches in ascending k followed by the labels call equal pnp_native_labels_ensemble on the same K members bit for
+ * bit, labels and counts; K = 1 equals pnp_native_labels.
+ * pnp_native_accumulate rejects what pnp_native_labels rejects (covered in the place of out, no gt / cm) and NULL sums as
+ * PNP_ERR_BAD_ARG.  pnp_native_accumulated_labels: NULL sums / covered / out, only one of gt / cm or a non-positive size are
+ * PNP_ERR_BAD_ARG; C outside [2, 8], a dimension above PNP_RS_MAX_DIM or m0*m1*m2 >= 2^31 are PNP_ERR_UNSUPPORTED.  On any error
+ * nothing is launched and the outputs are untouched.  Each voxel is read and written by one thread per launch, so a sequence of
+ * calls is bit-identical when repeated. */
+int pnp_native_accumulate(const float* scores, int n0, int n1, int n2, int C, const float* map, int m0, int m1, int m2, float* sums,
+                          uint8_t* covered, void* stream);
+int pnp_native_accumulated_labels(const float* sums, const uint8_t* covered, int m0, int m1, int m2, int C, uint8_t* out,
+                                  const uint8_t* gt, long long* cm, void* stream);
+
 /* ---- evaluation: largest connected component per class (components3d.cu) ------------------------------------------------------
  * The usual clean-up of a segmentation (nnU-Net's post-processing): every structure is one connected body, so only the largest
  * 3-D connected component of each class is kept and the rest is set to background.  labels, out and gt are uint8 C-order
@@ -501,6 +524,16 @@ int pnp_native_labels_ensemble(const float* scores, int K, int n0, int n1, int n
 int pnp_largest_components_workspace(int n0, int n1, int n2, int C, int connectivity, long long* bytes /* host */);
 int pnp_largest_components(const uint8_t* labels, int n0, int n1, int n2, int C, int connectivity, uint8_t* out, const uint8_t* gt,
                            long long* cm, long long* stats, void* ws, long long ws_bytes, void* stream);
+
+/* ---- per-class voxel count and bounding box (components3d.cu) -------------------------------------------------------------
+ * labels: uint8 C-order [n0][n1][n2] on the device; labels >= C count as class 0.  out: int64 [C][7] on the device,
+ *   out[c] = (count, lo0, hi0, lo1, hi1, lo2, hi2): the number of voxels of class c and the inclusive index bounds of them along
+ *   each axis; an empty class gives (0, n0, -1, n1, -1, n2, -1).  The call initialises out itself.
+ * Two launches: the empty boxes, then per-thread counts and bounds reduced per warp and folded in by integer atomics, so out is an
+ * exact function of the input and repeated calls are bit-identical.
+ * NULL labels / out or a non-positive size are PNP_ERR_BAD_ARG; C outside [2, 8] or n0*n1*n2 >= 2^31 are PNP_ERR_UNSUPPORTED.  On
+ * any error nothing is launched and out is untouched. */
+int pnp_label_boxes(const uint8_t* labels, int n0, int n1, int n2, int C, long long* out, void* stream);
 
 #ifdef __cplusplus
 }

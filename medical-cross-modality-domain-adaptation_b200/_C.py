@@ -125,6 +125,9 @@ SIGNATURES = {
     "pnp_smooth_noise_field": [c_ull, c_ull, c_int, c_int, c_int, c_int, P, c_int, c_float, c_float, c_float, P, P, P],
     "pnp_native_labels": [P, c_int, c_int, c_int, c_int, P, c_int, c_int, c_int, P, P, P, P],
     "pnp_native_labels_ensemble": [P, c_int, c_int, c_int, c_int, c_int, P, c_int, c_int, c_int, P, P, P, P],
+    "pnp_native_accumulate": [P, c_int, c_int, c_int, c_int, P, c_int, c_int, c_int, P, P, P],
+    "pnp_native_accumulated_labels": [P, P, c_int, c_int, c_int, c_int, P, P, P, P],
+    "pnp_label_boxes": [P, c_int, c_int, c_int, c_int, P, P],
     "pnp_largest_components_workspace": [c_int, c_int, c_int, c_int, c_int, P],
     "pnp_largest_components": [P, c_int, c_int, c_int, c_int, c_int, P, P, P, P, P, c_ll, P],
 }

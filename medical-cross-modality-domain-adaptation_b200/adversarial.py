@@ -555,19 +555,30 @@ class Trainer(object):
                                        flip_correction, save_result, shuffle=True, write_cm=True, surface_metrics=surface_metrics,
                                        hd_percentile=hd_percentile)
 
-    def test_native(self, pairs, output_path, hd_percentile=None, largest_component=None, checkpoints=None, tta=None):
+    def test_native(self, pairs, output_path, hd_percentile=None, largest_component=None, checkpoints=None, tta=None,
+                    locate=None):
         """every raw (image, label) pair segmented on its own grid by the adapted CT stream (native.run): writes
         <output_path>/native_pred/<name>_label.nii.gz and native.csv, prints per-organ Dice and ASSD / HD in mm -> per-subject
         results.  `hd_percentile` q also scores the q-th percentile HD in mm (native.csv column <organ>_hd<q>_mm).
         `largest_component` 6 or 26 keeps only the largest connected component of each organ before scoring and writing.
         `checkpoints` (.npz paths, each restored before its members' frames are predicted) and `tta` ((theta_deg, scale_r,
         scale_c, shift_r, shift_c) test-time transforms) ensemble the prediction (native.Ensemble; the critics need not be
-        stored); every variable holds its value from before the call again when it returns."""
+        stored); every variable holds its value from before the call again when it returns.  `locate` (a localise.Calibration or
+        its JSON path) crops every subject at the heart box the network locates without its labels (native.run)."""
         from . import native
         # restore loads a key 'x:0' as variable x
         ensemble = native.trainer_ensemble(self.net, checkpoints, tta, native.SLOT_KEYWORDS + ("cls",), strip_suffix=True)
         return native.run(self._ct_logits, pairs, output_path, self.net.batch_size, self.num_cls or self.net.n_class,
-                          hd_percentile, largest_component, ensemble)
+                          hd_percentile, largest_component, ensemble, locate)
+
+    def segment_native(self, images, output_path, calibration, largest_component=None, checkpoints=None, tta=None):
+        """unlabelled scans located with `calibration` and segmented on their own grid by the adapted CT stream (native.segment):
+        writes <output_path>/native_pred/<name>_label.nii.gz and located.csv; `largest_component`, `checkpoints` and `tta` as
+        test_native takes them"""
+        from . import native
+        ensemble = native.trainer_ensemble(self.net, checkpoints, tta, native.SLOT_KEYWORDS + ("cls",), strip_suffix=True)
+        return native.segment(self._ct_logits, images, output_path, self.net.batch_size, self.num_cls or self.net.n_class,
+                              calibration, largest_component, ensemble)
 
     def sample_metric_stddev(self, sample_eval_list):
         """adversarial.py:1054-1084"""

@@ -9,6 +9,8 @@
 //   select    per class: number of roots, atomicMax of (size << 32) | (0xFFFFFFFF - root)  -> the largest, first in C order
 //   write     out[v] = class if v's root is its class's kept root, else 0; stats kept / removed; cm[gt][out]
 // Every quantity is an integer, so out, stats and cm are exact functions of the input and repeated calls are bit-identical.
+// pnp_label_boxes (native.py's heart localisation) reduces each class's voxel count and bounding box: per-thread registers, a warp
+// reduction, then one integer atomic per warp, class and field.
 #include "common.cuh"
 #include "../../include/pnp_b200.h"
 
@@ -201,6 +203,67 @@ lcc_write_kernel(const uint8_t* labels, int C, long long total, const int* __res
   }
 }
 
+// out[c] = (count, lo0, hi0, lo1, hi1, lo2, hi2): the empty box (0, n0, -1, n1, -1, n2, -1) that the atomics shrink onto the voxels
+__global__ void __launch_bounds__(THREADS) box_init_kernel(int n0, int n1, int n2, int C, long long* __restrict__ out) {
+  pnp_pdl_enter();
+  const int t = threadIdx.x, f = t % 7;
+  if (t < 7 * C) out[t] = f == 0 ? 0 : (f % 2 == 0 ? -1 : (f == 1 ? n0 : (f == 3 ? n1 : n2)));
+}
+
+// Each thread keeps every class's count and bounds in registers (the class selects its slot through an unrolled compare, so no
+// local memory); after the grid-stride loop, which every thread leaves, each warp reduces them with __reduce_*_sync and lane 0
+// folds the warp's result into out with one integer atomic per non-empty class and field.
+__global__ void __launch_bounds__(THREADS)
+label_boxes_kernel(const uint8_t* __restrict__ labels, int n1, int n2, int C, long long total, long long* __restrict__ out) {
+  pnp_pdl_enter();
+  unsigned cnt[8];
+  int lo0[8], hi0[8], lo1[8], hi1[8], lo2[8], hi2[8];
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    cnt[c] = 0u;
+    lo0[c] = lo1[c] = lo2[c] = 0x7FFFFFFF;
+    hi0[c] = hi1[c] = hi2[c] = -1;
+  }
+  for (long long i = (long long)blockIdx.x * THREADS + threadIdx.x; i < total; i += (long long)gridDim.x * THREADS) {
+    const int v = (int)i;
+    const int l = class_of(__ldg(labels + v), C);
+    const int row = v / n2;
+    const int k = v - row * n2, j = row % n1, i0 = row / n1;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      if (c == l) {
+        cnt[c] += 1u;
+        lo0[c] = min(lo0[c], i0);
+        hi0[c] = max(hi0[c], i0);
+        lo1[c] = min(lo1[c], j);
+        hi1[c] = max(hi1[c], j);
+        lo2[c] = min(lo2[c], k);
+        hi2[c] = max(hi2[c], k);
+      }
+    }
+  }
+  const unsigned full = 0xffffffffu;
+  const bool lead = (threadIdx.x & 31) == 0;
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    if (c >= C) break;
+    const unsigned n = __reduce_add_sync(full, cnt[c]);
+    const int a0 = __reduce_min_sync(full, lo0[c]), b0 = __reduce_max_sync(full, hi0[c]);
+    const int a1 = __reduce_min_sync(full, lo1[c]), b1 = __reduce_max_sync(full, hi1[c]);
+    const int a2 = __reduce_min_sync(full, lo2[c]), b2 = __reduce_max_sync(full, hi2[c]);
+    if (lead && n) {
+      long long* o = out + 7 * c;
+      atomicAdd((u64*)o, (u64)n);
+      atomicMin(o + 1, (long long)a0);
+      atomicMax(o + 2, (long long)b0);
+      atomicMin(o + 3, (long long)a1);
+      atomicMax(o + 4, (long long)b1);
+      atomicMin(o + 5, (long long)a2);
+      atomicMax(o + 6, (long long)b2);
+    }
+  }
+}
+
 inline long long align256(long long b) { return (b + 255) & ~255LL; }
 
 // bytes = 2 A(4N) + 256: parent and size (int32 per voxel), then the 8 per-class keys
@@ -248,5 +311,15 @@ extern "C" int pnp_largest_components(const uint8_t* labels, int n0, int n1, int
   PNP_CUDA(pnp_launch(lcc_select_kernel, grid, THREADS, 0, st, labels, C, N, (const int*)parent, (const int*)size, best, stats));
   PNP_CUDA(pnp_launch(lcc_write_kernel, grid, THREADS, 0, st, labels, C, N, (const int*)parent, (const u64*)best, out, gt, stats,
                       cm));
+  return PNP_OK;
+}
+
+extern "C" int pnp_label_boxes(const uint8_t* labels, int n0, int n1, int n2, int C, long long* out, void* stream) {
+  if (!labels || !out || n0 <= 0 || n1 <= 0 || n2 <= 0) return PNP_ERR_BAD_ARG;
+  if (C < 2 || C > 8 || (long long)n0 * n1 * n2 >= (1LL << 31)) return PNP_ERR_UNSUPPORTED;
+  const long long N = (long long)n0 * n1 * n2;
+  cudaStream_t st = (cudaStream_t)stream;
+  PNP_CUDA(pnp_launch(box_init_kernel, 1, THREADS, 0, st, n0, n1, n2, C, out));
+  PNP_CUDA(pnp_launch(label_boxes_kernel, grid_for(N, THREADS * 4), THREADS, 0, st, labels, n1, n2, C, N, out));
   return PNP_OK;
 }

@@ -4,7 +4,9 @@
 // without record files or a host-to-device image copy.  A grid-stride gather: the writes are coalesced along the NHWC index,
 // the reads follow the sampled coordinates.  The way back (native.py): pnp_native_labels samples the class scores of the prepared
 // grid at every voxel of the subject's native grid with the same taps and lerps, and labels it by their argmax;
-// pnp_native_labels_ensemble sums the scores of several members (checkpoints, test-time transforms) first.  The opt-in
+// pnp_native_labels_ensemble sums the scores of several members (checkpoints, test-time transforms) first, and
+// pnp_native_accumulate / pnp_native_accumulated_labels do the same for any number of members, one launch per member into a
+// native-grid sum volume, then one argmax launch.  The opt-in
 // augmentations: pnp_smooth_noise_field draws smoothed Philox noise fields (elastic displacement, bias gain) and
 // pnp_resample_planes_aug resamples at the displaced pixels and applies gain, contrast and offset.
 #include "common.cuh"
@@ -101,16 +103,18 @@ resample_planes_kernel(const float* __restrict__ vol, const uint8_t* __restrict_
 }
 
 // Native voxel q = (i m1 + j) m2 + k: trilinear class scores at its prepared-grid coordinate, first-max argmax, and with gt the
-// (truth, prediction) pair in a per-CTA histogram flushed by one global atomic per non-zero bin.
-// ENS = false is pnp_native_labels: one member, its map held in registers (K and stride unused).
+// (truth, prediction) pair in a per-CTA histogram flushed by one global atomic per non-zero bin.  One body serves three kernels:
+// ENS = false, ACC = false is pnp_native_labels: one member, its map held in registers (K and stride unused).
 // ENS = true is pnp_native_labels_ensemble: member k's scores start at scores + k stride and its map at map + 12 k; the maps are
 // staged in shared memory once per CTA, and the class scores of the members covering the voxel are summed in ascending k (the
 // first one taken as it is) before the argmax.
-template <bool ENS>
-__global__ void __launch_bounds__(256)
-native_labels_kernel(const float* __restrict__ scores, int n0, int n1, int n2, int C, const float* __restrict__ map, int m1, int m2,
-                     long long total, uint8_t* __restrict__ out, const uint8_t* __restrict__ gt, long long* __restrict__ cm, int K,
-                     long long stride) {
+// ACC = true is pnp_native_accumulate: one member as pnp_native_labels samples it, its class scores stored into sums[q][.] where
+// out[q] (the coverage flags) is 0 -- out[q] is then set to 1 -- and added to them elsewhere (gt, cm, K and stride unused).
+template <bool ENS, bool ACC>
+__device__ __forceinline__ void native_labels_body(const float* __restrict__ scores, int n0, int n1, int n2, int C,
+                                                   const float* __restrict__ map, int m1, int m2, long long total,
+                                                   uint8_t* __restrict__ out, const uint8_t* __restrict__ gt, long long* __restrict__ cm,
+                                                   int K, long long stride, float* __restrict__ sums) {
   __shared__ unsigned int hist[64];
   __shared__ float maps[ENS ? 12 * PNP_NATIVE_MAX_MEMBERS : 1];
   pnp_pdl_enter();
@@ -153,6 +157,8 @@ native_labels_kernel(const float* __restrict__ scores, int n0, int n1, int n2, i
         const float* p11 = member + (long long)((b0 * n1 + b1) * n2) * C;
         const int o0 = a2 * C, o1 = b2 * C;
         float top = 0.f;
+        float* s = ACC ? sums + (long long)q * C : nullptr;      // 64-bit: m0 m1 m2 C may reach 2^31
+        const bool first = ACC && out[q] == 0;
 #pragma unroll
         for (int c = 0; c < (ENS ? 8 : C); ++c) {     // ENS unrolls to 8 classes and stops at C
           if (ENS && c >= C) break;
@@ -161,13 +167,16 @@ native_labels_kernel(const float* __restrict__ scores, int n0, int n1, int n2, i
           const float v10 = lerp_rn(__ldg(p10 + o0 + c), __ldg(p10 + o1 + c), f2);
           const float v11 = lerp_rn(__ldg(p11 + o0 + c), __ldg(p11 + o1 + c), f2);
           const float v = lerp_rn(lerp_rn(v00, v01, f1), lerp_rn(v10, v11, f1), f0);
-          if (ENS) {
+          if (ACC) {
+            s[c] = first ? v : __fadd_rn(s[c], v);             // the first covering member is taken as it is
+          } else if (ENS) {
             sum[c] = covered ? __fadd_rn(sum[c], v) : v;     // the first covering member is taken as it is
           } else if (c == 0 || v > top) {       // strictly greater: the lowest index wins a tie
             top = v;
             best = c;
           }
         }
+        if (ACC && first) out[q] = 1;
         covered = true;
       }
     }
@@ -177,6 +186,63 @@ native_labels_kernel(const float* __restrict__ scores, int n0, int n1, int n2, i
       for (int c = 1; c < 8; ++c) {
         if (c < C && sum[c] > top) {     // strictly greater: the lowest index wins a tie
           top = sum[c];
+          best = c;
+        }
+      }
+    }
+    if (ACC) continue;
+    out[q] = (uint8_t)best;
+    if (cm) {
+      int g = __ldg(gt + q);
+      if (g >= C) g = 0;
+      atomicAdd(&hist[g * C + best], 1u);
+    }
+  }
+  if (cm) {
+    __syncthreads();
+    if (threadIdx.x < C * C && hist[threadIdx.x])
+      atomicAdd((unsigned long long*)cm + threadIdx.x, (unsigned long long)hist[threadIdx.x]);
+  }
+}
+
+template <bool ENS>
+__global__ void __launch_bounds__(256)
+native_labels_kernel(const float* __restrict__ scores, int n0, int n1, int n2, int C, const float* __restrict__ map, int m1, int m2,
+                     long long total, uint8_t* __restrict__ out, const uint8_t* __restrict__ gt, long long* __restrict__ cm, int K,
+                     long long stride) {
+  native_labels_body<ENS, false>(scores, n0, n1, n2, C, map, m1, m2, total, out, gt, cm, K, stride, nullptr);
+}
+
+// pnp_native_accumulate: covered[q] is read and written by the one thread that samples voxel q
+__global__ void __launch_bounds__(256)
+native_accumulate_kernel(const float* __restrict__ scores, int n0, int n1, int n2, int C, const float* __restrict__ map, int m1, int m2,
+                         long long total, float* __restrict__ sums, uint8_t* __restrict__ covered) {
+  native_labels_body<false, true>(scores, n0, n1, n2, C, map, m1, m2, total, covered, nullptr, nullptr, 1, 0, sums);
+}
+
+// pnp_native_accumulated_labels: the first maximum of each covered voxel's sums, 0 where nothing covers it, with
+// pnp_native_labels' (truth, prediction) counts
+__global__ void __launch_bounds__(256)
+native_accumulated_labels_kernel(const float* __restrict__ sums, const uint8_t* __restrict__ covered, int C, long long total,
+                                 uint8_t* __restrict__ out, const uint8_t* __restrict__ gt, long long* __restrict__ cm) {
+  __shared__ unsigned int hist[64];
+  pnp_pdl_enter();
+  if (cm) {
+    if (threadIdx.x < 64) hist[threadIdx.x] = 0u;
+    __syncthreads();
+  }
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const unsigned q = (unsigned)i;
+    int best = 0;
+    if (__ldg(covered + q)) {
+      const float* sum = sums + (long long)q * C;       // 64-bit: m0 m1 m2 C may reach 2^31
+      float top = __ldg(sum);
+#pragma unroll
+      for (int c = 1; c < 8; ++c) {
+        if (c >= C) break;
+        const float v = __ldg(sum + c);
+        if (v > top) {                   // strictly greater: the lowest index wins a tie (pnp_native_labels_ensemble's rule)
+          top = v;
           best = c;
         }
       }
@@ -327,6 +393,14 @@ int launch_native(const float* scores, int K, int n0, int n1, int n2, int C, con
   return PNP_OK;
 }
 
+// the checks of the accumulator pair: sums [m0][m1][m2][C] may hold 2^31 floats or more (64-bit offsets), the voxel count may not
+int check_accumulated(const float* sums, const uint8_t* covered, int m0, int m1, int m2, int C) {
+  if (!sums || !covered || m0 <= 0 || m1 <= 0 || m2 <= 0) return PNP_ERR_BAD_ARG;
+  if (C < 2 || C > 8) return PNP_ERR_UNSUPPORTED;
+  if (m0 > PNP_RS_MAX_DIM || m1 > PNP_RS_MAX_DIM || m2 > PNP_RS_MAX_DIM || !count_below_2_31({m0, m1, m2})) return PNP_ERR_UNSUPPORTED;
+  return PNP_OK;
+}
+
 }  // namespace
 
 extern "C" int pnp_resample_planes(const float* vol, const uint8_t* cls, int n0, int n1, int n2, const float* mats, int B, int H, int W,
@@ -375,4 +449,27 @@ extern "C" int pnp_native_labels_ensemble(const float* scores, int K, int n0, in
   if (rc != PNP_OK) return rc;
   if (K > PNP_NATIVE_MAX_MEMBERS) return PNP_ERR_UNSUPPORTED;
   return launch_native<true>(scores, K, n0, n1, n2, C, maps, m0, m1, m2, out, gt, cm, stream);
+}
+
+extern "C" int pnp_native_accumulate(const float* scores, int n0, int n1, int n2, int C, const float* map, int m0, int m1, int m2,
+                                     float* sums, uint8_t* covered, void* stream) {
+  if (!sums) return PNP_ERR_BAD_ARG;
+  const int rc = check_native(scores, n0, n1, n2, C, map, m0, m1, m2, covered, nullptr, nullptr);
+  if (rc != PNP_OK) return rc;
+  const long long total = (long long)m0 * m1 * m2;
+  PNP_CUDA(pnp_launch(native_accumulate_kernel, grid_for(total, 256 * 4), 256, 0, (cudaStream_t)stream, scores, n0, n1, n2, C, map, m1,
+                      m2, total, sums, covered));
+  return PNP_OK;
+}
+
+extern "C" int pnp_native_accumulated_labels(const float* sums, const uint8_t* covered, int m0, int m1, int m2, int C, uint8_t* out,
+                                             const uint8_t* gt, long long* cm, void* stream) {
+  if (!out || (!gt) != (!cm)) return PNP_ERR_BAD_ARG;
+  const int rc = check_accumulated(sums, covered, m0, m1, m2, C);
+  if (rc != PNP_OK) return rc;
+  const long long total = (long long)m0 * m1 * m2;
+  if (cm) PNP_CUDA(cudaMemsetAsync(cm, 0, sizeof(long long) * C * C, (cudaStream_t)stream));
+  PNP_CUDA(pnp_launch(native_accumulated_labels_kernel, grid_for(total, 256 * 4), 256, 0, (cudaStream_t)stream, sums, covered, C, total,
+                      out, gt, cm));
+  return PNP_OK;
 }

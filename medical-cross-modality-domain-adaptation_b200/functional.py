@@ -1195,6 +1195,61 @@ def native_labels(scores, vmap, shape, gt=None, out=None):
     return out, cm
 
 
+class NativeAccumulator(object):
+    """Native-grid labels of any number of predictions (include/pnp_b200.h, "native-grid labels of any number of predictions"):
+    fp32 sums [m0, m1, m2, C] and uint8 coverage flags [m0, m1, m2] on the device, zeroed once here.  `add(scores, vmap)` is one
+    pnp_native_accumulate launch (scores fp32 [n0, n1, n2, C], vmap fp32 [12], both on the device); `labels(gt=None, out=None)` one
+    pnp_native_accumulated_labels launch -> (labels uint8 [m0, m1, m2], confusion counts int64 [C, C] (rows = truth) or None), the
+    labels pnp_native_labels_ensemble gives for the same predictions in the same order."""
+
+    def __init__(self, shape, num_cls, device=None):
+        self.shape = tuple(int(s) for s in shape)
+        self.C = int(num_cls)
+        device = rt.device() if device is None else device
+        self.sums = torch.zeros(self.shape + (self.C,), dtype=torch.float32, device=device)
+        self.covered = torch.zeros(self.shape, dtype=torch.uint8, device=device)
+        self.count = 0
+
+    def add(self, scores, vmap):
+        scores, vmap = scores.contiguous(), vmap.contiguous()
+        n0, n1, n2, C = scores.shape
+        if C != self.C or tuple(vmap.shape) != (12,):
+            raise ValueError("NativeAccumulator.add: scores [n0, n1, n2, %d] and vmap [12] expected, got %s and %s" % (
+                self.C, tuple(scores.shape), tuple(vmap.shape)))
+        m0, m1, m2 = self.shape
+        call("pnp_native_accumulate", ptr(scores), n0, n1, n2, C, ptr(vmap), m0, m1, m2, ptr(self.sums), ptr(self.covered),
+             rt.stream())
+        self.count += 1
+
+    def labels(self, gt=None, out=None):
+        m0, m1, m2 = self.shape
+        if out is None:
+            out = torch.empty(self.shape, dtype=torch.uint8, device=self.sums.device)
+        cm = None
+        if gt is not None:
+            gt = gt.contiguous()
+            if tuple(gt.shape) != self.shape or gt.dtype != torch.uint8:
+                raise ValueError("NativeAccumulator.labels: gt must be uint8 %s, got %s %s" % (self.shape, tuple(gt.shape), gt.dtype))
+            cm = torch.empty(self.C, self.C, dtype=torch.int64, device=self.sums.device)
+        call("pnp_native_accumulated_labels", ptr(self.sums), ptr(self.covered), m0, m1, m2, self.C, ptr(out), ptr(gt), ptr(cm),
+             rt.stream())
+        return out, cm
+
+
+BOX_FIELDS = ("count", "lo0", "hi0", "lo1", "hi1", "lo2", "hi2")
+
+
+def label_boxes(labels, num_cls):
+    """host int64 [num_cls, 7]: per class (count, lo0, hi0, lo1, hi1, lo2, hi2) of `labels` (uint8 [n0, n1, n2] on the device;
+    labels >= num_cls count as class 0), one pnp_label_boxes call; an empty class is (0, n0, -1, n1, -1, n2, -1)"""
+    if not isinstance(labels, torch.Tensor) or not labels.is_cuda or labels.dtype != torch.uint8 or labels.dim() != 3:
+        raise ValueError("label_boxes: labels must be a uint8 3-D tensor on the device")
+    labels = labels.contiguous()
+    out = torch.empty(int(num_cls), 7, dtype=torch.int64, device=labels.device)
+    call("pnp_label_boxes", ptr(labels), *labels.shape, int(num_cls), ptr(out), rt.stream())
+    return out.cpu().numpy()
+
+
 COMPONENT_STATS = ("components", "kept", "removed")
 
 

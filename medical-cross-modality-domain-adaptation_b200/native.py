@@ -31,8 +31,13 @@ for the prepared test split), and a label map of that same scan comes out:
   <organ>_dice_raw / _components / _removed after those with the post-processing, and `members` and <organ>_dice_first after
   all the others for an ensemble).
 
-The crop is the ground-truth heart box, as for the prepared test split: a native-grid score is that of a prediction made inside a
-ground-truth region of interest."""
+* optional heart localisation (run(locate=), segment; localise.py): the crop is the box the network itself locates in the scan,
+  without its labels -- a sliding-window seed pass, then re-cropping around the predicted heart until the crop stops moving --,
+  and the subject is predicted from that crop as above.  With labels, native.csv adds windows, iterations, converged, box_iou
+  and box_err_mm (the located against the ground-truth whole-heart box) after all the others; segment writes located.csv.
+
+Otherwise the crop is the ground-truth heart box, as for the prepared test split: a native-grid score is then that of a
+prediction made inside a ground-truth region of interest."""
 import contextlib
 import logging
 import os
@@ -51,6 +56,7 @@ from .prepare_data import _upload
 CSV_COLUMNS = ("dice", "assd_mm", "hd_mm", "border_pred", "border_gt")
 COMPONENT_COLUMNS = ("dice_raw", "components", "removed")      # per organ, with the largest-component post-processing
 ENSEMBLE_COLUMNS = ("dice_first",)                              # per organ, after `members`, for an ensemble of K > 1
+LOCATE_COLUMNS = ("windows", "iterations", "converged", "box_iou", "box_err_mm")   # after all others, for located subjects
 CONNECTIVITIES = (6, 26)
 MAX_MEMBERS = 16                                                # PNP_NATIVE_MAX_MEMBERS
 SLOT_KEYWORDS = ("Adam", "RMS")                                 # optimizer slot names: never needed by a prediction
@@ -154,11 +160,11 @@ def ground_truth(label_path):
 
 
 def native_prediction(subject, scores, gt, T=None):
-    """(labels uint8 [native shape] on the device, confusion counts int64 [C, C] on the host): one pnp_native_labels launch.
-    T: the in-plane transform the score volume was predicted through (None: unaugmented)."""
+    """(labels uint8 [native shape] on the device, confusion counts int64 [C, C] on the host, None without gt): one
+    pnp_native_labels launch.  T: the in-plane transform the score volume was predicted through (None: unaugmented)."""
     vmap = torch.from_numpy(member_map32(subject, T)).to(scores.device)
     labels, cm = F.native_labels(scores, vmap, subject.native_shape, gt)
-    return labels, cm.cpu().numpy()
+    return labels, (None if cm is None else cm.cpu().numpy())
 
 
 def check_members(K):
@@ -279,15 +285,19 @@ def check_connectivity(largest_component):
     return None if largest_component is None else int(largest_component)
 
 
-def evaluate_subject(logits_fn, image_path, label_path, out_dir, batch_size, num_cls, hd_percentile=None, largest_component=None,
+def evaluate_subject(logits_fn, subject, label_path, out_dir, batch_size, num_cls, hd_percentile=None, largest_component=None,
                      ensemble=None):
     """one subject end to end -> dict: subject, dice, jaccard, cm, the surface_distances fields, the prediction's path.
+    `subject` is an image path (cropped at its ground-truth heart box: preprocess.Subject(subject, label_path)) or an already built
+    preprocess.Subject (e.g. one located by localise.locate).  `label_path` None: nothing is scored, and the dict holds subject,
+    path and counts (voxels per class of the written labels) only.
     `largest_component` 6 or 26 keeps only the largest connected component of each class of the native labels (in place, before
     they are scored or written) and adds largest_component, dice_raw (before it), components (in the raw labels), kept and
     removed (voxels), each [num_cls].  `ensemble` (an Ensemble) predicts through its members; with K > 1 the labels are those of
     pnp_native_labels_ensemble and members (K) and dice_first (member 0 alone, without post-processing) are added."""
     largest_component = check_connectivity(largest_component)
-    s = preprocess.Subject(image_path, label_path)
+    s = subject if isinstance(subject, preprocess.Subject) else preprocess.Subject(subject, label_path)
+    scored = label_path is not None
     gt = None
     ens = {}
     if ensemble is None or ensemble.K == 1:
@@ -295,23 +305,35 @@ def evaluate_subject(logits_fn, image_path, label_path, out_dir, batch_size, num
         if ensemble is not None:
             ensemble.load(path)
         scores = predict_scores(s, logits_fn, batch_size, num_cls, T)
-        gt = ground_truth(label_path)
+        gt = ground_truth(label_path) if scored else None
         labels, cm = native_prediction(s, scores, gt, T)
     else:
         logging.info("%s: %d ensemble members, score buffer %.1f MB", s.name, ensemble.K,
                      workspace_bytes(s, ensemble.K, num_cls) / 1e6)
         scores, vmap = ensemble_scores(s, logits_fn, batch_size, num_cls, ensemble)
-        gt = ground_truth(label_path)
+        gt = ground_truth(label_path) if scored else None
         labels, cm = F.native_labels(scores, vmap, s.native_shape, gt)
-        _, cm_first = F.native_labels(scores[0], vmap[0], s.native_shape, gt)
-        cm = cm.cpu().numpy()
-        ens = {"members": ensemble.K, "dice_first": _dice(cm_first.cpu().numpy())}
+        ens = {"members": ensemble.K}
+        if scored:
+            _, cm_first = F.native_labels(scores[0], vmap[0], s.native_shape, gt)
+            cm = cm.cpu().numpy()
+            ens["dice_first"] = _dice(cm_first.cpu().numpy())
     del scores
     post = {}
     if largest_component is not None:
-        post["dice_raw"] = _dice(cm)
+        if scored:
+            post["dice_raw"] = _dice(cm)
         labels, stats, cm = F.largest_components(labels, num_cls, largest_component, gt=gt, out=labels)
         post.update(stats, largest_component=largest_component)
+    if not scored:
+        counts = F.label_boxes(labels, num_cls)[:, 0]
+        labels = labels.cpu().numpy()
+        res = dict(subject=s.name, counts=counts, path=write_prediction(s, labels, out_dir, num_cls))
+        res.update(post)
+        res.update(ens)
+        logging.info("%s: native grid %s, %d prepared frames, voxels per class %s (not scored)", s.name, s.native_shape, s.D,
+                     counts.tolist())
+        return res
     labels, gt = labels.cpu().numpy(), gt.cpu().numpy()
     res = surface_mm(s, labels, gt, num_cls, hd_percentile)
     res.update(subject=s.name, dice=_dice(cm), jaccard=_jaccard(cm), cm=cm, path=write_prediction(s, labels, out_dir, num_cls))
@@ -326,6 +348,24 @@ def evaluate_subject(logits_fn, image_path, label_path, out_dir, batch_size, num
     if ens:
         logging.info("%s: Dice of member 0 alone %s", s.name, np.round(res["dice_first"], 4))
     return res
+
+
+def locate_subject(logits_fn, image_path, batch_size, num_cls, calibration, ensemble=None):
+    """localise.locate on one image with the network as restored (an ensemble's first checkpoint, no transform) -> Located"""
+    from . import localise
+    if ensemble is not None:
+        ensemble.load(ensemble.checkpoints[0])
+    return localise.locate(image_path, lambda s: predict_scores(s, logits_fn, batch_size, num_cls), calibration, num_cls)
+
+
+def located_fields(found, scan_spacing, truth=None):
+    """the LOCATE_COLUMNS of a Located (and, with the ground-truth whole-heart box, box_iou and box_err_mm)"""
+    from . import localise
+    out = {"windows": found.windows, "iterations": found.iterations, "converged": found.converged}
+    if truth is not None:
+        out["box_iou"] = localise.box_iou(found.subject.box, truth)
+        out["box_err_mm"] = localise.face_distance_mm(found.subject.box, truth, scan_spacing)
+    return out
 
 
 def _largest_component(results):
@@ -344,11 +384,20 @@ def _members(results):
     return ks.pop() if ks else None
 
 
+def _located(results):
+    """whether the subjects' dicts carry the localisation's fields; every subject must agree"""
+    ks = {"windows" in r for r in results}
+    if len(ks) > 1:
+        raise ValueError("some subjects were located and some were not")
+    return ks.pop() if ks else False
+
+
 def write_csv(path, results, num_cls):
     """one row per subject: subject, then <organ>_<column> for every organ and CSV_COLUMNS entry (NaN: organ absent),
     <organ>_hd<q>_mm when the subjects were scored with a percentile, after all of those <organ>_<column> for every organ and
     COMPONENT_COLUMNS entry when the labels were post-processed to their largest components, and after everything else, for an
-    ensemble of K > 1 members, `members` and <organ>_<column> for every organ and ENSEMBLE_COLUMNS entry"""
+    ensemble of K > 1 members, `members` and <organ>_<column> for every organ and ENSEMBLE_COLUMNS entry, then LOCATE_COLUMNS for
+    subjects cropped at a located box"""
     names = evaluation._organ_names(num_cls)
     q = evaluation._hd_percentile(results)
     cols = CSV_COLUMNS if q is None else CSV_COLUMNS + (evaluation.pct_name(q) + "_mm",)
@@ -357,6 +406,9 @@ def write_csv(path, results, num_cls):
     members = _members(results)
     if members is not None:
         extra += ["members"] + ["%s_%s" % (names[c], k) for c in range(1, num_cls) for k in ENSEMBLE_COLUMNS]
+    located = _located(results)
+    if located:
+        extra += list(LOCATE_COLUMNS)
     with open(path, "w") as f:
         f.write(",".join(["subject"] + ["%s_%s" % (names[c], k) for c in range(1, num_cls) for k in cols] + extra) + "\n")
         for r in results:
@@ -372,30 +424,117 @@ def write_csv(path, results, num_cls):
             if members is not None:
                 row.append(str(int(r["members"])))
                 row += [repr(float(r["dice_first"][c])) for c in range(1, num_cls)]
+            if located:
+                row += [str(int(r["windows"])), str(int(r["iterations"])), str(bool(r["converged"])), repr(float(r["box_iou"])),
+                        repr(float(r["box_err_mm"]))]
             f.write(",".join(row) + "\n")
     return path
 
 
-def run(logits_fn, pairs, output_path, batch_size, num_cls, hd_percentile=None, largest_component=None, ensemble=None):
+def run(logits_fn, pairs, output_path, batch_size, num_cls, hd_percentile=None, largest_component=None, ensemble=None,
+        locate=None):
     """every (image, label) pair through evaluate_subject; writes <output_path>/native_pred/*.nii.gz and native.csv, prints the
     per-organ mean and spread of Dice / Jaccard and of ASSD / HD (and the `hd_percentile`-th percentile HD) in mm -> the
     per-subject results.  `largest_component` 6 or 26: every prediction is first reduced to the largest connected component of
     each class (evaluate_subject); the files and printed figures are then those of the post-processed labels.  `ensemble` (an
     Ensemble): every subject is predicted by its members, and every graph variable holds its value from before the call again
-    when it returns."""
+    when it returns.  `locate` (a localise.Calibration or its JSON path): every subject is cropped at the box localise.locate finds
+    without its labels, which are read only afterwards, to score the prediction and the box (native.csv adds LOCATE_COLUMNS); a
+    subject in which nothing is located is logged and left out."""
     largest_component = check_connectivity(largest_component)
     pred_dir = os.path.join(output_path, "native_pred")
     os.makedirs(pred_dir, exist_ok=True)
+    if locate is not None:
+        from . import localise
+        locate = localise.as_calibration(locate)
     if ensemble is not None:
         logging.info("native-grid ensemble: %d checkpoint(s) x %d transform(s) = %d members", len(ensemble.checkpoints),
                      len(ensemble.transforms), ensemble.K)
+    results = []
     with (ensemble.preserved() if ensemble is not None else contextlib.nullcontext()):
-        results = [evaluate_subject(logits_fn, im, lb, pred_dir, batch_size, num_cls, hd_percentile, largest_component, ensemble)
-                   for im, lb in pairs]
+        for im, lb in pairs:
+            if locate is None:
+                results.append(evaluate_subject(logits_fn, im, lb, pred_dir, batch_size, num_cls, hd_percentile, largest_component,
+                                                ensemble))
+                continue
+            found = locate_subject(logits_fn, im, batch_size, num_cls, locate, ensemble)
+            if found.subject is None:
+                logging.error("%s: no heart located; the subject is left out of native.csv", preprocess.subject_name(im))
+                continue
+            truth = localise.truth_box(found.subject, lb)
+            res = evaluate_subject(logits_fn, found.subject, lb, pred_dir, batch_size, num_cls, hd_percentile, largest_component,
+                                   ensemble)
+            res.update(located_fields(found, found.subject.spacing, truth))
+            results.append(res)
     write_csv(os.path.join(output_path, "native.csv"), results, num_cls)
     evaluation.sample_metric_stddev([(r["dice"], r["jaccard"]) for r in results], num_cls)
     evaluation.surface_metric_stddev(results, num_cls, units="mm")
     return results
+
+
+def write_located_csv(path, results, num_cls):
+    """located.csv: subject, windows, iterations, converged, the located coronal box (voxels, then its extent in mm per axis), px,
+    D, and per organ the predicted volume in mL (voxels x native voxel volume); a subject in which nothing was located has empty
+    box, px, D and volume fields"""
+    names = evaluation._organ_names(num_cls)
+    axes = ("row", "col", "slice")
+    head = (["subject", "windows", "iterations", "converged"] + ["box_%s_%s" % (a, e) for a in axes for e in ("lo", "hi")] +
+            ["box_%s_mm" % a for a in axes] + ["px_mm", "D"] + ["%s_ml" % names[c] for c in range(1, num_cls)])
+    with open(path, "w") as f:
+        f.write(",".join(head) + "\n")
+        for r in results:
+            row = [str(r["subject"]), str(int(r["windows"])), str(int(r["iterations"])), str(bool(r["converged"]))]
+            if r.get("box") is None:
+                row += [""] * (len(head) - len(row))
+            else:
+                row += [str(int(v)) for lohi in r["box"] for v in lohi]
+                row += [repr(float(x)) for x in r["box_mm"]]
+                row += [repr(float(r["px"])), str(int(r["D"]))]
+                row += [repr(float(r["volume_ml"][c])) for c in range(1, num_cls)]
+            f.write(",".join(row) + "\n")
+    return path
+
+
+def segment(logits_fn, images, output_path, batch_size, num_cls, calibration, largest_component=None, ensemble=None):
+    """unlabelled scans segmented on their own grid: each image is located (localise.locate with `calibration`, a
+    localise.Calibration or its JSON path), cropped at the located box and predicted as evaluate_subject predicts a labelled one
+    (`largest_component`, `ensemble` as there).  Writes <output_path>/native_pred/<name>_label.nii.gz and located.csv
+    (write_located_csv) -> the per-subject dicts.  No label is read."""
+    from . import localise
+    largest_component = check_connectivity(largest_component)
+    calibration = localise.as_calibration(calibration)
+    pred_dir = os.path.join(output_path, "native_pred")
+    os.makedirs(pred_dir, exist_ok=True)
+    results = []
+    with (ensemble.preserved() if ensemble is not None else contextlib.nullcontext()):
+        for im in images:
+            found = locate_subject(logits_fn, im, batch_size, num_cls, calibration, ensemble)
+            res = {"subject": preprocess.subject_name(im), "box": None}
+            if found.subject is None:
+                logging.error("%s: no heart located; nothing written", res["subject"])
+            else:
+                s = found.subject
+                res = evaluate_subject(logits_fn, s, None, pred_dir, batch_size, num_cls, None, largest_component, ensemble)
+                res.update(box=s.box, box_mm=[(hi - lo + 1) * s.spacing[a] for a, (lo, hi) in enumerate(s.box)], px=s.px, D=s.D,
+                           volume_ml=res["counts"] * float(np.prod(native_spacing(s))) / 1000.0)
+            res.update(located_fields(found, None))
+            results.append(res)
+    write_located_csv(os.path.join(output_path, "located.csv"), results, num_cls)
+    return results
+
+
+def read_images(path):
+    """a text file of one image path per line -> [path]; blank lines are skipped"""
+    out = []
+    with open(path) as f:
+        for ln in f:
+            parts = ln.split()
+            if not parts:
+                continue
+            if len(parts) != 1:
+                raise ValueError("%s: expected one image path per line, got %r" % (path, ln.strip()))
+            out.append(parts[0])
+    return out
 
 
 def trainer_ensemble(net, checkpoints, tta, skip_keywords, strip_suffix):
@@ -435,7 +574,14 @@ def main(argv=None):
     ap.add_argument("--checkpoint", required=True, nargs="+", metavar="CKPT",
                     help=".npz checkpoint(s) of that trainer; several are ensembled (their class probabilities summed at every "
                          "native voxel before the argmax; native.csv columns members and <organ>_dice_first)")
-    ap.add_argument("--pairs", required=True, help="text file of `image_path label_path` lines (as prepare_data.py reads)")
+    ap.add_argument("--pairs", default=None, help="text file of `image_path label_path` lines (as prepare_data.py reads)")
+    ap.add_argument("--images", default=None, metavar="LIST",
+                    help="text file of one unlabelled image path per line: segmented without scoring (needs --locate; writes "
+                         "located.csv)")
+    ap.add_argument("--locate", default=None, metavar="CALIBRATION",
+                    help="crop each scan at the heart box the network itself locates (localiser JSON of calibrate_localiser.py) "
+                         "instead of the ground-truth box; with --pairs native.csv adds windows, iterations, converged, box_iou "
+                         "and box_err_mm")
     ap.add_argument("--out", required=True)
     ap.add_argument("--batch-size", type=int, default=8, help="frames per forward call")
     ap.add_argument("--hd-percentile", type=float, default=None, metavar="Q",
@@ -449,17 +595,32 @@ def main(argv=None):
     ap.add_argument("--tta-scales", type=float, nargs="+", default=[1.0], metavar="S",
                     help="test-time augmentation: isotropic in-plane scales (within [%g, %g])" % preprocess.SCALE_RANGE)
     a = ap.parse_args(argv)
+    if (a.pairs is None) == (a.images is None):
+        ap.error("give exactly one of --pairs and --images")
+    if a.images is not None and a.locate is None:
+        ap.error("--images needs --locate: an unlabelled scan has no ground-truth box to crop at")
+    if a.images is not None and a.hd_percentile is not None:
+        ap.error("--hd-percentile scores against labels; --images has none")
     logging.basicConfig(level=logging.INFO)
     tta = [(r, sc, sc, 0.0, 0.0) for r in a.tta_rotations for sc in a.tta_scales]
     check_members(len(a.checkpoint) * len(tta))       # before any work
     transforms = tta_transforms(tta)
     tta = None if len(transforms) == 1 and transforms[0] is None else tta      # the identity alone: today's single prediction
     checkpoints = None if len(a.checkpoint) == 1 else a.checkpoint
+    if a.locate is not None:
+        from . import localise
+        calibration = localise.Calibration.load(a.locate)          # before any work
     trainer = build_trainer(a.trainer, a.checkpoint[0] if checkpoints is None else None, a.batch_size)
     os.makedirs(a.out, exist_ok=True)
     post = {} if a.largest_component is None else {"largest_component": a.largest_component}
     if checkpoints is not None or tta is not None:
         post.update(checkpoints=checkpoints, tta=tta)
+    if a.images is not None:
+        results = trainer.segment_native(read_images(a.images), a.out, calibration, **post)
+        print(os.path.join(a.out, "located.csv"))
+        return results
+    if a.locate is not None:
+        post["locate"] = calibration
     results = trainer.test_native(preprocess.read_pairs(a.pairs), a.out, a.hd_percentile, **post)
     print(os.path.join(a.out, "native.csv"))
     return results

@@ -143,6 +143,10 @@ def heart_box(heart):
     return box
 
 
+class ConstantIntensity(ValueError):
+    """intensity_stats of a box whose clipped intensities are constant"""
+
+
 def intensity_stats(raw_box):
     """(p98, mu, sigma) of the raw voxels inside the heart box: linear 98th percentile, then the mean and population standard
     deviation of min(x, p98), in fp64"""
@@ -151,7 +155,7 @@ def intensity_stats(raw_box):
     clipped = np.minimum(x, p98)
     mu, sigma = float(clipped.mean()), float(clipped.std())
     if not sigma > 0:
-        raise ValueError("constant intensity inside the heart box: the volume cannot be z-scored")
+        raise ConstantIntensity("constant intensity inside the heart box: the volume cannot be z-scored")
     return p98, mu, sigma
 
 
@@ -215,29 +219,76 @@ def subject_name(image_path):
     return b[:-len("_image")] if b.endswith("_image") else b
 
 
-class Subject(object):
-    """One prepared (image, label) pair.  `vol` (fp32) and `cls` (uint8) are the uploaded sub-volume in slice-major order
-    [slice, row, column] of the coronal frame, so a plane's gathers run along contiguous rows.  `D` slices of 256 x 256 pixels of
-    `px` mm; the heart covers slices j_lo .. j_hi (each with both neighbours inside the D)."""
+class Scan(object):
+    """One loaded image in the coronal frame: `raw` (a view of the stored voxels), its `spacing` in mm, `coronal_affine`, and the
+    native grid a prediction is written back onto (`native_shape`, `native_affine`, `frame`: coronal voxel -> native voxel).
+    Loading is the slow part of a subject; the heart localisation (localise.py) crops many subjects out of one Scan."""
 
-    def __init__(self, image_path, label_path, margin=MARGIN, reach_px=REACH_PX):
+    def __init__(self, image_path):
+        self.path = str(image_path)
         self.name = subject_name(image_path)
-        im, lb = nifti.load(image_path), nifti.load(label_path)
-        if im.shape != lb.shape or len(im.shape) != 3:
-            raise ValueError("%s: image %s and label %s must be equal-shaped 3-D volumes" % (self.name, im.shape, lb.shape))
-        raw, spacing, self.coronal_affine, angle = to_coronal(im.get_data(), im.get_affine())
-        # the native grid, for predictions written back onto it (native.py): shape, affine, and coronal voxel -> native voxel
+        self.image = im = nifti.load(image_path)
+        if len(im.shape) != 3:
+            raise ValueError("%s: image %s must be a 3-D volume" % (self.name, im.shape))
+        self.raw, spacing, self.coronal_affine, angle = to_coronal(im.get_data(), im.get_affine())
         self.native_shape = tuple(int(n) for n in im.shape)
         self.native_affine = np.asarray(im.get_affine(), np.float64)
         self.frame = coronal_frame(self.native_affine, self.native_shape)[2]
+        self.spacing = np.asarray(spacing, np.float64)
+        self.angle = angle
+
+
+class Subject(object):
+    """One prepared (image, label) pair.  `vol` (fp32) and `cls` (uint8) are the uploaded sub-volume in slice-major order
+    [slice, row, column] of the coronal frame, so a plane's gathers run along contiguous rows.  `D` slices of 256 x 256 pixels of
+    `px` mm; the heart covers slices j_lo .. j_hi (each with both neighbours inside the D).  `box` is the coronal voxel box the
+    crop was set from: the whole-heart label box for Subject(image, label), any box for Subject.from_box(scan, box) (no labels:
+    `cls` is class 0 everywhere)."""
+
+    def __init__(self, image_path, label_path, margin=MARGIN, reach_px=REACH_PX):
+        scan = self._geometry(image_path)
+        cls_all, box = self._labels(scan, label_path)
+        self._crop(scan, cls_all, box, margin, reach_px)
+
+    @classmethod
+    def from_box(cls, scan, box, margin=MARGIN, reach_px=REACH_PX):
+        """the subject of `scan` (a Scan or an image path) cropped at the coronal voxel box [(lo, hi)] * 3 exactly as a
+        ground-truth box would crop it, without labels"""
+        self = cls.__new__(cls)
+        scan = self._geometry(scan)
+        self._crop(scan, np.zeros(scan.raw.shape, np.uint8), [(int(lo), int(hi)) for lo, hi in box], margin, reach_px)
+        return self
+
+    def _geometry(self, image):
+        """step 1: the image, its coronal frame and native grid"""
+        scan = image if isinstance(image, Scan) else Scan(image)
+        self.name = scan.name
+        self.coronal_affine = scan.coronal_affine
+        # the native grid, for predictions written back onto it (native.py): shape, affine, and coronal voxel -> native voxel
+        self.native_shape = scan.native_shape
+        self.native_affine = scan.native_affine
+        self.frame = scan.frame
+        return scan
+
+    def _labels(self, scan, label_path):
+        """step 2: class ids in the coronal frame and the whole-heart box of the label volume"""
+        lb = nifti.load(label_path)
+        if scan.native_shape != tuple(int(n) for n in lb.shape):
+            raise ValueError("%s: image %s and label %s must be equal-shaped 3-D volumes" % (self.name, scan.native_shape, lb.shape))
         cls_all, heart, unknown = map_labels(lb.get_data())
-        cls_all = to_coronal(cls_all, im.get_affine())[0]
-        heart = to_coronal(heart, im.get_affine())[0]
+        affine = scan.image.get_affine()
+        cls_all = to_coronal(cls_all, affine)[0]
+        heart = to_coronal(heart, affine)[0]
         if unknown:
             logging.warning("%s: %d label voxels hold values outside the MMWHS set (mapped to background)", self.name, unknown)
-        logging.info("%s: largest angle between a voxel axis and its world axis %.3f degrees", self.name, angle)
-        self.spacing = s = np.asarray(spacing, np.float64)
-        box = heart_box(heart)
+        return cls_all, heart_box(heart)
+
+    def _crop(self, scan, cls_all, box, margin, reach_px):
+        """step 3: the crop, intensity statistics and uploaded sub-volume set from the coronal voxel box"""
+        raw = scan.raw
+        logging.info("%s: largest angle between a voxel axis and its world axis %.3f degrees", self.name, scan.angle)
+        self.spacing = s = scan.spacing
+        self.box = box
         ext = np.array([(hi - lo + 1) * s[a] for a, (lo, hi) in enumerate(box)])
         self.centre = c = np.array([(lo + hi) / 2.0 for lo, hi in box])
         self.px = px = (1.0 + 2.0 * margin) * max(ext[0], ext[1]) / SIZE

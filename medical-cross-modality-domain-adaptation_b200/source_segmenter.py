@@ -394,18 +394,29 @@ class Trainer(object):
         return evaluation.run_protocol(self, self._logits, self.num_cls, output_path, "test_pred", flip_correction, save_result,
                                        shuffle=False, write_cm=False, surface_metrics=surface_metrics, hd_percentile=hd_percentile)
 
-    def test_native(self, pairs, output_path, hd_percentile=None, largest_component=None, checkpoints=None, tta=None):
+    def test_native(self, pairs, output_path, hd_percentile=None, largest_component=None, checkpoints=None, tta=None,
+                    locate=None):
         """every raw (image, label) pair segmented on its own grid (native.run): writes <output_path>/native_pred/<name>_label.nii.gz
         and native.csv, prints per-organ Dice and ASSD / HD in mm -> per-subject results.  `hd_percentile` q also scores the q-th
         percentile HD in mm (native.csv column <organ>_hd<q>_mm).  `largest_component` 6 or 26 keeps only the largest connected
         component of each organ before scoring and writing.  `checkpoints` (.npz paths, each restored before its members' frames
         are predicted) and `tta` ((theta_deg, scale_r, scale_c, shift_r, shift_c) test-time transforms) ensemble the prediction
-        (native.Ensemble); every variable holds its value from before the call again when it returns."""
+        (native.Ensemble); every variable holds its value from before the call again when it returns.  `locate` (a
+        localise.Calibration or its JSON path) crops every subject at the heart box the network locates without its labels."""
         from . import native
         # restore loads exact variable names only
         ensemble = native.trainer_ensemble(self.net, checkpoints, tta, native.SLOT_KEYWORDS, strip_suffix=False)
         return native.run(self._logits, pairs, output_path, self.net.batch_size, self.num_cls, hd_percentile, largest_component,
-                          ensemble)
+                          ensemble, locate)
+
+    def segment_native(self, images, output_path, calibration, largest_component=None, checkpoints=None, tta=None):
+        """unlabelled scans located with `calibration` and segmented on their own grid (native.segment): writes
+        <output_path>/native_pred/<name>_label.nii.gz and located.csv; `largest_component`, `checkpoints` and `tta` as
+        test_native takes them"""
+        from . import native
+        ensemble = native.trainer_ensemble(self.net, checkpoints, tta, native.SLOT_KEYWORDS, strip_suffix=False)
+        return native.segment(self._logits, images, output_path, self.net.batch_size, self.num_cls, calibration,
+                              largest_component, ensemble)
 
     def sample_metric_stddev(self, sample_eval_list):
         """source_segmenter.py:634-664"""
