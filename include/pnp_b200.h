@@ -257,6 +257,19 @@ int pnp_segloss_finalize(const double* acc, long long P, int C, float* out, floa
 /* dlogits = g_wce * d wce/dlogits + g_dice * d dice/dlogits */
 int pnp_segloss_bwd(const float* logits, const float* y, const float* coef, const float* g_wce, const float* g_dice,
                     float* dlogits, long long P, int C, void* stream);
+/* Mean Shannon entropy of the per-pixel softmax of logits [P, C] (fp32, NHWC with P = B*H*W), TENT's test-time objective.
+ * Per pixel, in fp32: m = max_c l_c; t_c = l_c - m; e_c = expf(t_c); s = sum_c e_c (ascending c); log p_c = t_c - logf(s);
+ * p_c = e_c / s; H_p = -sum_c p_c * log p_c.  For finite logits every log p_c is finite: a saturated pixel gives H = 0, not NaN,
+ * and nothing is clamped.  L = (1/P) sum_p H_p; dL/dl_j = -(1/P) * p_j * (log p_j + H_p).
+ *   pnp_entropy_reduce:   acc[0] += sum_p H_p; acc[1 + c] += sum_p p_c (fp64 accumulation; acc[1 + C] zeroed by the caller).
+ *   pnp_entropy_finalize: out[0] = (float)(acc[0] / P) = L; out[1 + c] = (float)(acc[1 + c] / P), the mean class probability
+ *                         (a diagnostic: it is not differentiated).
+ *   pnp_entropy_bwd:      dlogits = g[0] * dL/dlogits computed as (-g[0] / (float)P) * (p_j * (log p_j + H_p)); g is a device
+ *                         scalar, so a captured graph reads it on every replay.
+ * 2 <= C <= 8 and P >= 1; NULL pointers or other sizes are PNP_ERR_BAD_ARG, and nothing is launched. */
+int pnp_entropy_reduce(const float* logits, long long P, int C, double* acc, void* stream);
+int pnp_entropy_finalize(const double* acc, long long P, int C, float* out, void* stream);
+int pnp_entropy_bwd(const float* logits, const float* g, float* dlogits, long long P, int C, void* stream);
 /* lib.py:96-110 + tf.confusion_matrix: counts[C*C] (confusion, rows = truth), from logits argmax vs one-hot y */
 int pnp_confusion(const float* logits, const float* y, long long P, int C, unsigned long long* counts, void* stream);
 /* lib._label_decomp (lib.py:75-92): int64 label map -> one-hot fp32 [P, C], on the device */

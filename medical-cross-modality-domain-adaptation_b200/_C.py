@@ -100,6 +100,9 @@ SIGNATURES = {
     "pnp_segloss_reduce": [P, P, c_ll, c_int, P, P],
     "pnp_segloss_finalize": [P, c_ll, c_int, P, P, P],
     "pnp_segloss_bwd": [P, P, P, P, P, P, c_ll, c_int, P],
+    "pnp_entropy_reduce": [P, c_ll, c_int, P, P],
+    "pnp_entropy_finalize": [P, c_ll, c_int, P, P],
+    "pnp_entropy_bwd": [P, P, P, c_ll, c_int, P],
     "pnp_confusion": [P, P, c_ll, c_int, P, P],
     "pnp_one_hot": [P, P, c_ll, c_int, P],
     "pnp_fc_fwd": [P, P, P, c_int, c_int, P],

@@ -647,6 +647,27 @@ class Trainer(object):
         fwd = lambda x: self.net.segment(x, "ct", 1.0, front_bn=True, joint_bn=(scope == "all"))
         return bnstats.recalibrate(self, ct_source, batches, bnstats.covered_statistics(covered), fwd)
 
+    def entropy_adaptation(self, lr=1e-4):
+        """an open tent.EntropyAdaptation of the DAM: gamma and beta of its 20 adapt_* batch norms train (batch statistics, keep_prob
+        1) in a fresh Adam over the G arena; groups 7-9 and the tail run as at inference, and no critic runs.  Closing it
+        resets the D / G mode, so the next d_step / g_step sets its own requires_grad flags again."""
+        from . import tent
+        covered = [v for v in self.g_vars if v.pnp_kind in ("bn_gamma", "bn_beta")]
+        fwd = lambda x: self.net.segment(x, "ct", 1.0, front_bn=True, joint_bn=False)["logits"]
+        return tent.EntropyAdaptation(self, self.g_arena, covered, fwd, lr, self.d_vars + self.g_vars,
+                                      on_close=lambda: setattr(self, "_mode", None))
+
+    def adapt_entropy(self, ct_source, steps, lr=1e-4, recalibrate_batches=200):
+        """TENT (tent.py; DESIGN 6.1): `steps` entropy-minimisation steps of the DAM's batch-norm gamma / beta on unlabelled
+        images from `ct_source` (.next() -> (images, labels), labels ignored; the network's batch size), then recalibrate_bn(
+        ct_source, recalibrate_batches, scope='dam').  The trainer's own optimizers and global_step are untouched; anything raising
+        puts the snapshotted variables back.  -> (covered variable names, history [steps, 1 + C] numpy, slice count).
+        ValueError: steps < 1, recalibrate_batches < 1, a non-positive lr or a wrong batch size; FloatingPointError: a
+        non-finite loss; NotImplementedError under data parallelism."""
+        from . import tent
+        return tent.adapt(self.entropy_adaptation, ct_source, steps, lr, recalibrate_batches,
+                          lambda src, n: self.recalibrate_bn(src, n, scope="dam"))
+
     def joint_step(self, mr_batch, ct_batch, keep_prob=0.75, ct_batch_g=None):
         """one full adversarial step (D update + clip, then G update); replays the captured graph when there is one.
         `ct_batch_g`: the fresh CT batch the reference dequeues for the generator update (adversarial.py:869-873);

@@ -879,13 +879,81 @@ image_summary_u8_kernel(ImgPlan plan, int n, long long HW, unsigned char* __rest
   }
 }
 
-__device__ __forceinline__ void stable_softmax(const float* l, int C, float* p) {
-  float mx = l[0];
+// the max-subtracted exponentials of stable_softmax: m = max_c l_c (returned in mx), e_c = expf(l_c - m), and their sum in
+// ascending c
+__device__ __forceinline__ float softmax_exp_sum(const float* l, int C, float* e, float& mx) {
+  mx = l[0];
   for (int c = 1; c < C; ++c) mx = fmaxf(mx, l[c]);
   float s = 0.f;
-  for (int c = 0; c < C; ++c) { p[c] = expf(l[c] - mx); s += p[c]; }
+  for (int c = 0; c < C; ++c) { e[c] = expf(l[c] - mx); s += e[c]; }
+  return s;
+}
+
+__device__ __forceinline__ void stable_softmax(const float* l, int C, float* p) {
+  float mx;
+  float s = softmax_exp_sum(l, C, p, mx);
   float inv = 1.f / s;
   for (int c = 0; c < C; ++c) p[c] *= inv;
+}
+
+// Shannon entropy of one pixel's softmax (TENT's objective), with its log-probabilities lp[] and probabilities p[]:
+// lp_c = (l_c - m) - logf(s), p_c = e_c / s, H = -sum_c p_c * lp_c (ascending c).  Every log-probability of a finite pixel is
+// finite, so a saturated pixel gives p_c * lp_c = 0 * finite and H = 0, never 0 * -inf.
+__device__ __forceinline__ float entropy_px(const float* l, int C, float* lp, float* p) {
+  float mx;
+  const float s = softmax_exp_sum(l, C, p, mx);
+  const float ls = logf(s);
+  float h = 0.f;
+  for (int c = 0; c < C; ++c) {
+    lp[c] = (l[c] - mx) - ls;
+    p[c] = p[c] / s;
+    h -= p[c] * lp[c];
+  }
+  return h;
+}
+
+__global__ void __launch_bounds__(256)
+entropy_reduce_kernel(const float* __restrict__ logits, long long P, int C, double* __restrict__ acc) {
+  pnp_pdl_enter();
+  __shared__ double s_acc[1 + kMaxC];
+  if (threadIdx.x < 1 + kMaxC) s_acc[threadIdx.x] = 0.0;
+  __syncthreads();
+  double d[1 + kMaxC];
+#pragma unroll
+  for (int i = 0; i < 1 + kMaxC; ++i) d[i] = 0.0;
+  for (long long p = (long long)blockIdx.x * 256 + threadIdx.x; p < P; p += (long long)gridDim.x * 256) {
+    float l[kMaxC], lp[kMaxC], pr[kMaxC];
+    for (int c = 0; c < C; ++c) l[c] = logits[p * C + c];
+    d[0] += (double)entropy_px(l, C, lp, pr);
+#pragma unroll
+    for (int c = 0; c < kMaxC; ++c)
+      if (c < C) d[1 + c] += (double)pr[c];
+  }
+#pragma unroll
+  for (int i = 0; i < 1 + kMaxC; ++i) {
+    double v = pnp_warp_sum_d(d[i]);
+    if ((threadIdx.x & 31) == 0) atomicAdd(&s_acc[i], v);
+  }
+  __syncthreads();
+  if (threadIdx.x <= C) atomicAdd(acc + threadIdx.x, s_acc[threadIdx.x]);
+}
+
+__global__ void entropy_finalize_kernel(const double* __restrict__ acc, long long P, int C, float* __restrict__ out) {
+  pnp_pdl_enter();
+  if (blockIdx.x == 0 && threadIdx.x <= C) out[threadIdx.x] = (float)(acc[threadIdx.x] / (double)P);
+}
+
+// dlogits_j = g * -(1/P) * p_j * (lp_j + H), g read from the device
+__global__ void __launch_bounds__(256)
+entropy_bwd_kernel(const float* __restrict__ logits, const float* __restrict__ g, float* __restrict__ dlogits, long long P, int C) {
+  pnp_pdl_enter();
+  const float k = -*g / (float)P;
+  for (long long p = (long long)blockIdx.x * 256 + threadIdx.x; p < P; p += (long long)gridDim.x * 256) {
+    float l[kMaxC], lp[kMaxC], pr[kMaxC];
+    for (int c = 0; c < C; ++c) l[c] = logits[p * C + c];
+    const float h = entropy_px(l, C, lp, pr);
+    for (int c = 0; c < C; ++c) dlogits[p * C + c] = k * (pr[c] * (lp[c] + h));
+  }
 }
 
 __global__ void __launch_bounds__(256)
@@ -1608,6 +1676,27 @@ extern "C" int pnp_segloss_bwd(const float* logits, const float* y, const float*
   if (!logits || !y || !coef || !dlogits || P <= 0 || C <= 0) return PNP_ERR_BAD_ARG;
   if (C > kMaxC) return PNP_ERR_UNSUPPORTED;
   pnp_launch(segloss_bwd_kernel, grid_for(P, 256 * 2), 256, 0, S_, logits, y, coef, g_wce, g_dice, dlogits, P, C);
+  PNP_LAUNCH_CHECK();
+  return PNP_OK;
+}
+
+extern "C" int pnp_entropy_reduce(const float* logits, long long P, int C, double* acc, void* stream) {
+  if (!logits || !acc || P < 1 || C < 2 || C > kMaxC) return PNP_ERR_BAD_ARG;
+  pnp_launch(entropy_reduce_kernel, grid_for(P, 256 * 2), 256, 0, S_, logits, P, C, acc);
+  PNP_LAUNCH_CHECK();
+  return PNP_OK;
+}
+
+extern "C" int pnp_entropy_finalize(const double* acc, long long P, int C, float* out, void* stream) {
+  if (!acc || !out || P < 1 || C < 2 || C > kMaxC) return PNP_ERR_BAD_ARG;
+  pnp_launch(entropy_finalize_kernel, 1, 32, 0, S_, acc, P, C, out);
+  PNP_LAUNCH_CHECK();
+  return PNP_OK;
+}
+
+extern "C" int pnp_entropy_bwd(const float* logits, const float* g, float* dlogits, long long P, int C, void* stream) {
+  if (!logits || !g || !dlogits || P < 1 || C < 2 || C > kMaxC) return PNP_ERR_BAD_ARG;
+  pnp_launch(entropy_bwd_kernel, grid_for(P, 256 * 2), 256, 0, S_, logits, g, dlogits, P, C);
   PNP_LAUNCH_CHECK();
   return PNP_OK;
 }

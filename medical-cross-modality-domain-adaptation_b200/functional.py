@@ -977,6 +977,40 @@ def seg_losses(logits, y):
     return _SegLossFn.apply(logits, y)
 
 
+class _EntropyLossFn(torch.autograd.Function):
+    """mean per-pixel softmax entropy of logits [..., C] (TENT's objective, pnp_entropy_*) and the mean class probability p-bar,
+    which is a diagnostic and not differentiated"""
+
+    @staticmethod
+    def forward(ctx, logits):
+        logits = logits.contiguous()
+        C = logits.shape[-1]
+        P = logits.numel() // C
+        acc = _zeros_f64(1 + C, logits.device)
+        call("pnp_entropy_reduce", ptr(logits), P, C, ptr(acc), rt.stream())
+        out = torch.empty(1 + C, dtype=torch.float32, device=logits.device)
+        call("pnp_entropy_finalize", ptr(acc), P, C, ptr(out), rt.stream())
+        ctx.save_for_backward(logits)
+        pbar = out[1:]
+        ctx.mark_non_differentiable(pbar)
+        return out[0], pbar
+
+    @staticmethod
+    def backward(ctx, g, _g_pbar):
+        logits, = ctx.saved_tensors
+        C = logits.shape[-1]
+        P = logits.numel() // C
+        dl = torch.empty_like(logits)
+        call("pnp_entropy_bwd", ptr(logits), ptr(g.contiguous()), ptr(dl), P, C, rt.stream())
+        return dl
+
+
+def entropy_loss(logits):
+    """-> (loss, pbar): the mean over pixels of -sum_c p_c log p_c of the softmax of `logits` [B, H, W, C], and the mean class
+    probability [C]"""
+    return _EntropyLossFn.apply(logits)
+
+
 def pixel_softmax2(logits):
     logits = logits.contiguous()
     C = logits.shape[-1]

@@ -224,6 +224,24 @@ class Trainer(object):
         fwd = lambda x: self.net.forward(x, 1.0, main_bn=True, adapt_bn=True)
         return bnstats.recalibrate(self, source, batches, covered, fwd)
 
+    def entropy_adaptation(self, lr=1e-4):
+        """an open tent.EntropyAdaptation: gamma and beta of all 30 batch norms train (batch statistics, keep_prob 1) in a fresh
+        Adam over the trainer's arena; every convolution weight stays fixed"""
+        from . import tent
+        covered = [v for v in self.trainables if v.pnp_kind in ("bn_gamma", "bn_beta")]
+        fwd = lambda x: self.net.forward(x, 1.0, main_bn=True, adapt_bn=True)
+        return tent.EntropyAdaptation(self, self.arena, covered, fwd, lr, self.trainables)
+
+    def adapt_entropy(self, source, steps, lr=1e-4, recalibrate_batches=200):
+        """TENT (tent.py; DESIGN 6.1): `steps` entropy-minimisation steps of every batch norm's gamma / beta on unlabelled images
+        from `source` (.next() -> (images, labels), labels ignored; the network's batch size), then recalibrate_bn(source,
+        recalibrate_batches).  The trainer's own optimizer and global_step are untouched; anything raising puts the snapshotted
+        variables back.  -> (covered variable names, history [steps, 1 + C] numpy, slice count).  ValueError: steps < 1,
+        recalibrate_batches < 1, a non-positive lr or a wrong batch size; FloatingPointError: a non-finite loss;
+        NotImplementedError under data parallelism."""
+        from . import tent
+        return tent.adapt(self.entropy_adaptation, source, steps, lr, recalibrate_batches, self.recalibrate_bn)
+
     def train_step_replay(self, batch_x, batch_y, keep_prob=0.75):
         if not rt.StepGraph.fits(self._graph, keep_prob):
             return self.train_step(batch_x, batch_y, keep_prob)
